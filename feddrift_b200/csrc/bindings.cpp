@@ -412,20 +412,19 @@ std::vector<Tensor> group_norm_bwd(Tensor x, Tensor dy, c10::optional<Tensor> w,
     return {dx, dg.sum(0), db.sum(0)};
 }
 
-Tensor gemm_tn_bias_act(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, bool out_fp32) {
-    TORCH_CHECK(A.is_cuda() && A.scalar_type() == torch::kBFloat16 && B.scalar_type() == torch::kBFloat16, "gemm_tn needs CUDA bf16 operands");
-    TORCH_CHECK(A.is_contiguous() && B.is_contiguous() && A.size(1) == B.size(1), "gemm_tn: A [M,K], B [N,K] contiguous");
-    c10::cuda::CUDAGuard guard(A.device());
-    const int M = (int)A.size(0), K = (int)A.size(1), N = (int)B.size(0);
+// D[M,N] = act(A·B + bias) on the wgmma GEMM.  The bias is cast to fp32; a bf16 output that gemm_launch splits over K gets its
+// fp32 accumulation workspace from the caching allocator (no driver call on the hot path).
+Tensor gemm_run(const Tensor& A, const void* B, int M, int N, int K, bool a_mn, bool b_mn, const c10::optional<Tensor>& bias, bool relu,
+                bool out_fp32, const char* what) {
     auto D = torch::empty({M, N}, A.options().dtype(out_fp32 ? torch::kFloat32 : torch::kBFloat16));
     const float* bp = nullptr;
     Tensor bias_f;
     if (bias.has_value() && bias->defined()) { bias_f = bias->to(torch::kFloat32).contiguous(); bp = bias_f.data_ptr<float>(); }
-    Tensor ws;   // fp32 split-K accumulator for bf16 outputs, from the caching allocator
+    Tensor ws;
     if (!out_fp32 && fdb::gemm_split_count(M, N, K) > 1) ws = torch::empty({M, N}, A.options().dtype(torch::kFloat32));
-    const int rc = fdb::gemm_launch(A.data_ptr(), B.data_ptr(), D.data_ptr(), bp, M, N, K, 0, 0, relu ? 1 : 0, out_fp32 ? 1 : 0, cur_stream(),
-                                    ws.defined() ? ws.data_ptr<float>() : nullptr);
-    CHECK_OK(rc, "gemm_tn (wgmma)");
+    const int rc = fdb::gemm_launch(A.data_ptr(), B, D.data_ptr(), bp, M, N, K, a_mn ? 1 : 0, b_mn ? 1 : 0, relu ? 1 : 0, out_fp32 ? 1 : 0,
+                                    cur_stream(), ws.defined() ? ws.data_ptr<float>() : nullptr);
+    CHECK_OK(rc, what);
     return D;
 }
 
@@ -437,16 +436,12 @@ Tensor gemm_bias_act(Tensor A, Tensor B, bool a_mn, bool b_mn, c10::optional<Ten
     c10::cuda::CUDAGuard guard(A.device());
     const int M = (int)A.size(a_mn ? 1 : 0), K = (int)A.size(a_mn ? 0 : 1), N = (int)B.size(b_mn ? 1 : 0);
     TORCH_CHECK(B.size(b_mn ? 0 : 1) == K, "gemm: reduction lengths differ");
-    auto D = torch::empty({M, N}, A.options().dtype(out_fp32 ? torch::kFloat32 : torch::kBFloat16));
-    const float* bp = nullptr;
-    Tensor bias_f;
-    if (bias.has_value() && bias->defined()) { bias_f = bias->to(torch::kFloat32).contiguous(); bp = bias_f.data_ptr<float>(); }
-    Tensor ws;
-    if (!out_fp32 && fdb::gemm_split_count(M, N, K) > 1) ws = torch::empty({M, N}, A.options().dtype(torch::kFloat32));
-    const int rc = fdb::gemm_launch(A.data_ptr(), B.data_ptr(), D.data_ptr(), bp, M, N, K, a_mn ? 1 : 0, b_mn ? 1 : 0, relu ? 1 : 0,
-                                    out_fp32 ? 1 : 0, cur_stream(), ws.defined() ? ws.data_ptr<float>() : nullptr);
-    CHECK_OK(rc, "gemm (wgmma)");
-    return D;
+    return gemm_run(A, B.data_ptr(), M, N, K, a_mn, b_mn, bias, relu, out_fp32, "gemm (wgmma)");
+}
+
+// D[M,N] = act(A[M,K] · B[N,K]ᵀ + bias)
+Tensor gemm_tn_bias_act(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, bool out_fp32) {
+    return gemm_bias_act(A, B, false, false, bias, relu, out_fp32);
 }
 
 // Batched weight-gradient GEMM (one launch for every pair): D[bt] [M, N] fp32 = A'[rows a_k0 + bt·a_kstride …+K, M]ᵀ · B'[rows b_k0 + bt·b_kstride …+K, N]
@@ -470,41 +465,8 @@ Tensor gemm_tn_bias_act_peer(Tensor A, int64_t b_ptr, int64_t N, c10::optional<T
     TORCH_CHECK(A.is_cuda() && A.scalar_type() == torch::kBFloat16 && A.is_contiguous(), "gemm_tn_peer: A must be CUDA bf16 [M,K]");
     TORCH_CHECK(b_ptr != 0 && N > 0, "gemm_tn_peer: null weight pointer");
     c10::cuda::CUDAGuard guard(A.device());
-    const int M = (int)A.size(0), K = (int)A.size(1);
-    auto D = torch::empty({M, N}, A.options().dtype(out_fp32 ? torch::kFloat32 : torch::kBFloat16));
-    const float* bp = nullptr;
-    Tensor bias_f;
-    if (bias.has_value() && bias->defined()) { bias_f = bias->to(torch::kFloat32).contiguous(); bp = bias_f.data_ptr<float>(); }
-    Tensor ws;
-    if (!out_fp32 && fdb::gemm_split_count(M, (int)N, K) > 1) ws = torch::empty({M, N}, A.options().dtype(torch::kFloat32));
-    const int rc = fdb::gemm_launch(A.data_ptr(), reinterpret_cast<const void*>(b_ptr), D.data_ptr(), bp, M, (int)N, K, 0, 0, relu ? 1 : 0,
-                                    out_fp32 ? 1 : 0, cur_stream(), ws.defined() ? ws.data_ptr<float>() : nullptr);
-    CHECK_OK(rc, "gemm_tn_peer (wgmma)");
-    return D;
-}
-
-// conv-as-GEMM helpers (csrc/conv_im2col.cu): x may be NCHW or channels_last — strides are passed through
-Tensor im2col_bf16(Tensor x, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t ph, int64_t pw) {
-    CHECK_CUDA_F32(x);
-    TORCH_CHECK(x.dim() == 4, "im2col: x must be [B, C, H, W]");
-    c10::cuda::CUDAGuard guard(x.device());
-    const int B = (int)x.size(0), C = (int)x.size(1), H = (int)x.size(2), W = (int)x.size(3);
-    const int Ho = (int)((H + 2 * ph - kh) / sh + 1), Wo = (int)((W + 2 * pw - kw) / sw + 1);
-    auto cols = torch::empty({(int64_t)B * Ho * Wo, (int64_t)C * kh * kw}, x.options().dtype(torch::kBFloat16));
-    CHECK_OK(fdb::im2col_bf16_launch(x.data_ptr<float>(), cols.data_ptr(), B, C, H, W, (int)kh, (int)kw, (int)sh, (int)sw, (int)ph, (int)pw,
-                                     Ho, Wo, x.stride(0), x.stride(1), x.stride(2), x.stride(3), cur_stream()), "im2col");
-    return cols;
-}
-Tensor col2im(Tensor dcols, int64_t B, int64_t C, int64_t H, int64_t W, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t ph,
-              int64_t pw) {
-    CHECK_CUDA_F32(dcols);
-    c10::cuda::CUDAGuard guard(dcols.device());
-    const int Ho = (int)((H + 2 * ph - kh) / sh + 1), Wo = (int)((W + 2 * pw - kw) / sw + 1);
-    TORCH_CHECK(dcols.is_contiguous() && dcols.size(0) == B * Ho * Wo && dcols.size(1) == C * kh * kw, "col2im: bad dcols shape");
-    auto dx = torch::empty({B, C, H, W}, dcols.options());
-    CHECK_OK(fdb::col2im_launch(dcols.data_ptr<float>(), dx.data_ptr<float>(), (int)B, (int)C, (int)H, (int)W, (int)kh, (int)kw, (int)sh,
-                                (int)sw, (int)ph, (int)pw, Ho, Wo, cur_stream()), "col2im");
-    return dx;
+    return gemm_run(A, reinterpret_cast<const void*>(b_ptr), (int)A.size(0), (int)N, (int)A.size(1), false, false, bias, relu, out_fp32,
+                    "gemm_tn_peer (wgmma)");
 }
 
 // Launch an instantiated CUDA graph on the current stream and (optionally) wait for it, with the GIL released: the
@@ -556,13 +518,9 @@ static fdb::LstmArgs lstm_args(const Tensor& params, const Tensor& row_off, cons
 }
 
 void lstm2_forward(Tensor params, Tensor row_off, std::vector<int64_t> offs, Tensor tokens, c10::optional<Tensor> gates,
-                   c10::optional<Tensor> cst, c10::optional<Tensor> hhist, Tensor hlast, int64_t E, c10::optional<Tensor> dbg) {
+                   c10::optional<Tensor> cst, c10::optional<Tensor> hhist, Tensor hlast, int64_t E) {
     c10::cuda::CUDAGuard guard(params.device());
     fdb::LstmArgs a = lstm_args(params, row_off, offs, tokens, gates, cst, hhist, hlast, E);
-    if (dbg.has_value() && dbg->defined()) {
-        TORCH_CHECK(dbg->is_cuda() && dbg->scalar_type() == torch::kInt64 && dbg->numel() >= 8, "dbg must be a CUDA int64[8] tensor");
-        a.dbg = reinterpret_cast<long long*>(dbg->data_ptr<int64_t>());
-    }
     CHECK_OK(fdb::lstm2_fwd_launch(a, (int)tokens.size(0), cur_stream()), "lstm2_fwd (cluster kernel)");
 }
 
@@ -840,8 +798,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("gemm_batched_mn", &gemm_batched_mn);
     m.def("gossip_mix_peer", &gossip_mix_peer);
     m.def("graph_launch_sync", &graph_launch_sync);
-    m.def("im2col_bf16", &im2col_bf16);
-    m.def("col2im", &col2im);
     m.def("lstm2_forward", &lstm2_forward);
     m.def("lstm2_backward", &lstm2_backward);
     m.def("lstm_head", &lstm_head);
@@ -852,12 +808,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("conv_tma_wgrad", &conv_tma_wgrad);
     m.def("conv_tma_dgrad", &conv_tma_dgrad);
     m.def("conv_cast_rows_bf16", &conv_cast_rows_bf16);
-    m.def("gemm_debug_counters", []() {
-        std::vector<int64_t> v(16);
-        cudaDeviceSynchronize();
-        CHECK_OK(fdb::gemm_debug_counters(reinterpret_cast<long long*>(v.data())), "gemm_debug_counters");
-        return v;
-    });
     m.def("conv_pack_t", &conv_pack_t);
     m.def("conv_igemm_dgrad", &conv_igemm_dgrad);
     m.def("conv_igemm_wgrad", &conv_igemm_wgrad);

@@ -26,7 +26,6 @@
 #include <cuda.h>
 
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <cuda_bf16.h>
 
@@ -52,9 +51,6 @@ struct GemmBatch { int batch, a_k0, a_kstride, b_k0, b_kstride; };
 //           MN-major 64-pixel × 64-channel im2col boxes, one per 64-wide column group of the N tile.
 struct ConvIm { int mode, S, cchunks, ntaps, Q, PQ, stride, pad_h, pad_w, flip, bcols; };
 
-// FDB_GEMM_DBG bit 3: CTA 0 accumulates SM-clock cycles per pipeline role / wait site (read back with gemm_debug_counters())
-__device__ long long g_gemm_dbg[16];
-
 template <int BN> struct GemmCfg {
     static constexpr uint32_t kStageBytesB = BN * BK * 2;
     static constexpr uint32_t kStagingBytes = 2 /*consumer warpgroups*/ * 2 /*double buffer*/ * 8192;   // 64 rows × 128 B per buffer
@@ -78,7 +74,7 @@ template <int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_d, void* __restrict__ D, const float* __restrict__ bias, int M, int N, int K,
-               int relu, int out_fp32, int splits, int tma_out, int a_mn, int b_mn, GemmBatch gb, ConvIm ci, int dbg) {
+               int relu, int out_fp32, int splits, int tma_out, int a_mn, int b_mn, GemmBatch gb, ConvIm ci) {
     using Cfg = GemmCfg<BN>;
     constexpr int STAGES = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
@@ -116,8 +112,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (warp == 0) {
         if (nkb > 0) {  // ===== TMA producer: the whole warp walks the loop (uniform control flow), one elected lane issues
             uint32_t it = 0;
-            const bool prof = (dbg & 8) && blockIdx.x == 0;
-            long long c_wait = 0, c_all0 = prof ? clock64() : 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int bt = tile / tiles_per_batch, rem = tile - bt * tiles_per_batch;
                 const int m_blk = rem % m_tiles, n_blk = rem / m_tiles;
@@ -135,12 +129,9 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 for (int kb = kb_lo; kb < kb_hi; ++kb, ++it) {
                     const int s = it % STAGES;
                     const uint32_t ph = (it / STAGES) & 1;
-                    const long long w0 = prof ? clock64() : 0;
-                    if (!(dbg & 16)) mbar_wait(empty_bar + s, ph ^ 1);   // bit 4 (with bit 0): free-running ring, no stage release
-                    if (prof) c_wait += clock64() - w0;
+                    mbar_wait(empty_bar + s, ph ^ 1);
                     uint8_t* sa = smem_a + s * kStageBytesA;
                     uint8_t* sb = smem_b + s * Cfg::kStageBytesB;
-                    if (dbg & 1) { if (elect_one()) mbar_arrive(full_bar + s); continue; }   // FDB_GEMM_DBG bit 0: pipeline without operand loads (timing study)
                     if (!elect_one()) continue;
                     if (ci.mode == 1) {
                         mbar_expect_tx(full_bar + s, kStageBytesA + Cfg::kStageBytesB);
@@ -186,15 +177,12 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     }
                 }
             }
-            if (prof && lane == 0) { g_gemm_dbg[0] = c_wait; g_gemm_dbg[1] = clock64() - c_all0; g_gemm_dbg[2] = it; }
         }
     } else if (warp >= 4 && nkb > 0) {
         // ===== consumer warpgroup wg: rows [64·wg, 64·wg + 64) of every tile; warp w of the group holds rows 16w + lane/4 (+8)
         const int wg = (warp >> 2) - 1, w = warp & 3, tg = threadIdx.x & 127;
         const int g8 = lane >> 2, c4 = lane & 3;
         uint32_t it = 0, chunk_it = 0;
-        const bool prof = (dbg & 8) && blockIdx.x == 0 && wg == 0 && w == 0;
-        long long c_wfull = 0, c_all0 = prof ? clock64() : 0;
         // the 64-row half of an A stage: K-major rows 64·wg… (64 × 128 B) or MN-major M group wg (64 K-rows × 128 B): 8 KB in both
         const uint64_t desc_a0 = (a_mn ? make_smem_desc_mn(smem_u32(smem_a)) : make_smem_desc(smem_u32(smem_a))) + (uint64_t)((wg * 8192) >> 4);
         const uint64_t desc_b0 = b_mn ? make_smem_desc_mn(smem_u32(smem_b)) : make_smem_desc(smem_u32(smem_b));
@@ -206,27 +194,24 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             for (int kb = 0; kb < nkb; ++kb, ++it) {
                 const int s = it % STAGES;
                 const uint32_t ph = (it / STAGES) & 1;
-                const long long f0 = prof ? clock64() : 0;
                 mbar_wait(full_bar + s, ph);
-                if (prof) c_wfull += clock64() - f0;
                 const uint64_t da0 = desc_a0 + (uint64_t)((s * kStageBytesA) >> 4);
                 const uint64_t db0 = desc_b0 + (uint64_t)((s * Cfg::kStageBytesB) >> 4);
-                if (!(dbg & 2)) {   // bit 1: no MMAs
-                    wgmma_fence();
-                    if (a_mn) {
-                        if (b_mn) gemm_kblock<BN, 1, 1>(d, da0, db0, kb == 0); else gemm_kblock<BN, 1, 0>(d, da0, db0, kb == 0);
-                    } else {
-                        if (b_mn) gemm_kblock<BN, 0, 1>(d, da0, db0, kb == 0); else gemm_kblock<BN, 0, 0>(d, da0, db0, kb == 0);
-                    }
-                    wgmma_commit();
-                    wgmma_wait<1>();   // the previous k-block's MMAs are complete: its stage may be refilled
+                wgmma_fence();
+                if (a_mn) {
+                    if (b_mn) gemm_kblock<BN, 1, 1>(d, da0, db0, kb == 0); else gemm_kblock<BN, 1, 0>(d, da0, db0, kb == 0);
+                } else {
+                    if (b_mn) gemm_kblock<BN, 0, 1>(d, da0, db0, kb == 0); else gemm_kblock<BN, 0, 0>(d, da0, db0, kb == 0);
                 }
-                if (s_prev >= 0 && !(dbg & 16)) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + s_prev); }
+                wgmma_commit();
+                wgmma_wait<1>();   // the previous k-block's MMAs are complete: its stage may be refilled
+                if (s_prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + s_prev); }
                 s_prev = s;
             }
             wgmma_wait<0>();
             fence_acc(d);
-            if (!(dbg & 16)) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + s_prev); }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar + s_prev);
 
             const int rbase = m_blk * BM + 64 * wg + 16 * w + g8;   // row of d[i] with (i/2)%2 == 0; +8 for the other half
             if (tma_out) {
@@ -292,7 +277,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     }
                     fence_proxy_async_smem();
                     named_bar_sync(1 + wg, 128);
-                    if (!(dbg & 4) && tg == 0) {   // bit 2: no output stores
+                    if (tg == 0) {
 #pragma unroll
                         for (int bx = 0; bx < 2; ++bx) {
                             const uint8_t* src = buf + bx * 4096;
@@ -323,7 +308,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 }
             }
         }
-        if (prof) { g_gemm_dbg[3] = c_wfull; g_gemm_dbg[5] = clock64() - c_all0; }
         if (tma_out && tg == 0) tma_store_wait_all();   // smem must outlive the in-flight bulk stores
     }
     __syncthreads();
@@ -457,15 +441,10 @@ static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, void* D, co
         if (cudaFuncSetAttribute(gemm_tn_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmemBytes) != cudaSuccess) return -3;
         attr_set = true;
     }
-    static const int dbg = getenv("FDB_GEMM_DBG") ? atoi(getenv("FDB_GEMM_DBG")) : 0;   // timing-study switches, results are garbage
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * gb.batch;
     dim3 grid(min(tiles, max(1, sms / splits)), 1, splits);
-    gemm_tn_kernel<BN><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ma, mb, md, D, bias, M, N, K, relu, out_fp32, splits, tma_out, a_mn, b_mn, gb, ci, dbg);
+    gemm_tn_kernel<BN><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ma, mb, md, D, bias, M, N, K, relu, out_fp32, splits, tma_out, a_mn, b_mn, gb, ci);
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
-}
-
-int gemm_debug_counters(long long* out16) {
-    return cudaMemcpyFromSymbol(out16, g_gemm_dbg, sizeof(long long) * 16) == cudaSuccess ? 0 : -4;
 }
 
 // number of K-splits gemm_launch will use for this problem (callers that want a bf16 output pre-allocate the fp32

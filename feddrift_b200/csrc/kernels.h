@@ -13,10 +13,6 @@ int weighted_average_launch(const float* rows, const float* w, int n, long long 
 int merge_axpby_launch(float* base_row, const float* second_row, float w1, float w2, long long P, cudaStream_t stream);
 int sq_diff_sum_launch(const float* a, const float* b, long long P, double* out, cudaStream_t stream);
 int gossip_mix_launch(const float* X, const float* Wm, int n, long long P, float* out, cudaStream_t stream);
-int im2col_bf16_launch(const float* x, void* cols, int B, int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw, int Ho, int Wo,
-                       long long sxb, long long sxc, long long sxh, long long sxw, cudaStream_t stream);
-int col2im_launch(const float* dcols, float* dx, int B, int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw, int Ho, int Wo,
-                  cudaStream_t stream);
 int gossip_mix_peer_launch(const long long* x_ptrs, const long long* flag_ptrs, const float* w, int P, int world, int rank,
                            unsigned* grid_sync, unsigned grid_base, unsigned epoch, int grid, long long timeout_ms, int* error_flag,
                            cudaStream_t stream);
@@ -81,7 +77,6 @@ int conv_tma_fwd_launch(const void* xb, const void* wq, float* y, const float* b
                         int Q, int pad, int stride, int dgrad, int relu, int groups, cudaStream_t stream);
 int conv_tma_wgrad_launch(const void* xb, const void* dyb, float* dw_ohwi, int N, int H, int W, int C, int Cout, int R, int S, int P, int Q,
                           int pad, int stride, int groups, long long gstride, cudaStream_t stream);
-int gemm_debug_counters(long long* out16);   // FDB_GEMM_DBG=8 cycle counters of CTA 0 (gemm_tc.cu)
 int conv_cast_rows_bf16_launch(const float* x, long long row_stride, void* out, int rows, long long n, cudaStream_t stream);
 // lstm_tc.cu : persistent cluster-resident 2-layer LSTM(256) forward / BPTT over many (client, model) pairs per launch
 struct LstmArgs {
@@ -97,7 +92,6 @@ struct LstmArgs {
     const float* dh2_last;        // [npairs, 16, 256] gradient wrt h2_{T-1}            (used when dh2_all == nullptr)
     const float* dh2_all;         // [npairs, T, 16, 256] gradient wrt every h2_t, or nullptr
     void* dgates;                 // [2, npairs, T, 16, 1024] bf16 pre-activation gate gradients (PyTorch row order)
-    long long* dbg;               // optional [8] per-segment SM-clock sums of the forward phase loop (CTA 0, thread 0)
     int T, E;
 };
 struct LstmHeadArgs {

@@ -174,20 +174,16 @@ lstm2_fwd_kernel(const __grid_constant__ LstmArgs a) {
     const bool keep = a.gates != nullptr;            // training: save gates / cell states for BPTT
     const bool keep_h = a.hhist != nullptr;
     const int unit = crank * U + l;
-    const bool dbg = a.dbg != nullptr && blockIdx.x == 0;
     const uint32_t bytes_each = NB * U * 2;
 
     if (grp == 2) {
         // =================================================== barrier warp: arm phase p's inbound barrier (the slices of phase p
         // land in hbar[p&1]) only after its previous phase completed
-        long long seg = 0, tprev = clock64();
         for (int p = 0; p <= T; ++p) {
             const bool doL1 = p < T, doL2 = p >= 1;
             if (p < T && elect_one()) mbar_expect_tx(hbar + (p & 1), CL * bytes_each * ((doL1 ? 1u : 0u) + (doL2 ? 1u : 0u)));
             if (p >= 1) mbar_wait_long(hbar + ((p - 1) & 1), ((p - 1) >> 1) & 1);   // h1_{p-1} (and h2_{p-2}) from all 8 CTAs
-            if (dbg) { const long long tn = clock64(); seg += tn - tprev; tprev = tn; }
         }
-        if (dbg && l == 0) { a.dbg[0] = seg; a.dbg[1] = 0; }
     } else {
         // =================================================== layer groups (layer = grp)
         const int layer = grp;
@@ -196,8 +192,6 @@ lstm2_fwd_kernel(const __grid_constant__ LstmArgs a) {
         __nv_bfloat16* hh_l = reinterpret_cast<__nv_bfloat16*>(a.hhist) + (size_t)(layer * NP + pair) * (T + 1) * NB * H;
         float* act = act_s + layer * 4 * NB * U;
         float creg[4] = {0.f, 0.f, 0.f, 0.f};
-        long long seg[4] = {0, 0, 0, 0}, tprev = clock64();
-        const bool dbgt = dbg && gt == 0 && layer == 0;
         // layer 1 runs in phases 0 … T-1 (time p), layer 2 in phases 1 … T (time p-1)
         const int p_lo = layer == 0 ? 0 : 1, p_hi = layer == 0 ? T - 1 : T;
         for (int p = p_lo; p <= p_hi; ++p) {
@@ -212,7 +206,6 @@ lstm2_fwd_kernel(const __grid_constant__ LstmArgs a) {
                 }
             }
             if (p >= 1) mbar_wait_long(hbar + ((p - 1) & 1), ((p - 1) >> 1) & 1);   // h1_{p-1} (and h2_{p-2}) from all 8 CTAs
-            if (dbgt) { const long long tn = clock64(); seg[0] += tn - tprev; tprev = tn; }
             // ---- GEMM: this warp's 32 gate rows × 16 batch columns
             {
                 float acc[2][2][4];
@@ -240,7 +233,6 @@ lstm2_fwd_kernel(const __grid_constant__ LstmArgs a) {
                         }
             }
             named_bar_sync(1 + layer, 128);
-            if (dbgt) { const long long tn = clock64(); seg[1] += tn - tprev; tprev = tn; }
             // ---- cell update for the own 32 units (unit l) × rows b = w + 4 i; stage the bf16 slice in operand layout
             __nv_bfloat16* st = stage + ((p & 1) * 2 + layer) * NB * U;
 #pragma unroll
@@ -271,7 +263,6 @@ lstm2_fwd_kernel(const __grid_constant__ LstmArgs a) {
             }
             fence_proxy_async_smem();   // generic-proxy writes (stage) → visible to the async proxy (bulk copy)
             named_bar_sync(1 + layer, 128);
-            if (dbgt) { const long long tn = clock64(); seg[2] += tn - tprev; tprev = tn; }
             // ---- all-gather: my 1-KB slice → every CTA's next-step operand buffer (incl. my own); lane d serves CTA d.
             //      (the last phase's h2_{T-1} is only needed as hlast, no exchange)
             if (p < T && gt < CL) {
@@ -280,9 +271,7 @@ lstm2_fwd_kernel(const __grid_constant__ LstmArgs a) {
                 const uint32_t dst = (layer == 0 ? smem_u32(H1s + (p & 1) * NB * H) : smem_u32(H2s + ((p + 1) & 1) * NB * H)) + crank * bytes_each;
                 bulk_copy_s2c(mapa_u32(dst, gt), smem_u32(st), bytes_each, mapa_u32(bar, gt));
             }
-            if (dbgt) { const long long tn = clock64(); seg[3] += tn - tprev; tprev = tn; }
         }
-        if (dbgt) for (int i = 0; i < 4; ++i) a.dbg[2 + i] = seg[i];
     }
     // ---- teardown: nobody may exit while peers still copy into its shared memory
     cluster.sync();

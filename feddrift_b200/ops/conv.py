@@ -13,9 +13,8 @@ forward, data gradient and weight gradient, NHWC activations end to end.  Two ke
 
 fp32 activations / master weights, bf16 tensor-core operands, fp32 accumulation; results are NCHW *views* with
 channels_last strides, so a chain of convolutions never transposes.  Shapes neither family covers (groups / dilation ≠ 1,
-1- or 3-channel stems) and CPU tensors use ``F.conv2d``.  ``FDB_CONV_IM2COL=1`` selects the round-1 explicit-im2col + GEMM
-formulation and ``FDB_NO_TMA_CONV=1`` the gather kernels everywhere (A/B measurements).  State-dict keys and the init law
-equal ``nn.Conv2d``'s.  Reference: cuDNN fp32 ``nn.Conv2d`` (``fedml_api/model/cv/cnn.py:110-117``).
+1- or 3-channel stems) and CPU tensors use ``F.conv2d``.  State-dict keys and the init law equal ``nn.Conv2d``'s.
+Reference: cuDNN fp32 ``nn.Conv2d`` (``fedml_api/model/cv/cnn.py:110-117``).
 """
 from __future__ import annotations
 
@@ -50,7 +49,7 @@ def igemm_eligible(cin: int, cout: int, stride, dilation, groups: int) -> bool:
 def tma_eligible(cin: int, stride, padding, ksize) -> bool:
     """The GEMM-mainloop path with the TMA-im2col producer: 64-channel K chunks, square filter, symmetric padding."""
     return (cin % 64 == 0 and ksize[0] == ksize[1] and padding[0] == padding[1] and stride[0] == stride[1] and 1 <= stride[0] <= 8
-            and padding[0] < 128 and os.environ.get("FDB_NO_TMA_CONV") != "1")
+            and padding[0] < 128)
 
 
 def _nhwc_bf16(ext, t: torch.Tensor, gate=None) -> torch.Tensor:
@@ -157,44 +156,6 @@ class _ConvIgemmFn(torch.autograd.Function):
         return gx, gw, gbias, None, None, None
 
 
-class _TcConvFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, weight, bias, stride, padding, relu: bool):
-        global TC_CONV_CALLS
-        TC_CONV_CALLS += 1
-        ext = _ext.load(required=True)
-        B, C, H, W = x.shape
-        Co, _, kh, kw = weight.shape
-        Ho, Wo = (H + 2 * padding[0] - kh) // stride[0] + 1, (W + 2 * padding[1] - kw) // stride[1] + 1
-        cols = ext.im2col_bf16(x.float(), kh, kw, stride[0], stride[1], padding[0], padding[1])
-        wb = weight.reshape(Co, -1).to(torch.bfloat16).contiguous()
-        y = ext.gemm_tn_bias_act(cols, wb, bias, bool(relu), True)           # [B·Ho·Wo, Co] fp32 == NHWC
-        ctx.save_for_backward(cols, wb, y if relu else None)
-        ctx.geom = (B, C, H, W, kh, kw, stride, padding, Ho, Wo, Co)
-        ctx.relu, ctx.has_bias = relu, bias is not None
-        return y.view(B, Ho, Wo, Co).permute(0, 3, 1, 2)                     # NCHW view, channels_last strides
-
-    @staticmethod
-    def backward(ctx, gy):
-        ext = _ext.load(required=True)
-        cols, wb, y = ctx.saved_tensors
-        B, C, H, W, kh, kw, stride, padding, Ho, Wo, Co = ctx.geom
-        g = gy.permute(0, 2, 3, 1).reshape(B * Ho * Wo, Co)                  # free when gy is channels_last
-        if ctx.relu:
-            g = g * (y > 0)
-        gb = g.to(torch.bfloat16).contiguous()
-        gx = gw = gbias = None
-        if ctx.needs_input_grad[0]:
-            dcols = ext.gemm_bias_act(gb, wb, False, True, None, False, True)               # dy · W  → [BHW, K] fp32
-            gx = ext.col2im(dcols, B, C, H, W, kh, kw, stride[0], stride[1], padding[0], padding[1])
-        if ctx.needs_input_grad[1]:
-            gw = ext.gemm_bias_act(gb, cols, True, True, None, False, True)                 # dyᵀ · cols, no transposes
-            gw = gw.view(Co, C, kh, kw)
-        if ctx.has_bias and ctx.needs_input_grad[2]:
-            gbias = g.sum(0)
-        return gx, gw, gbias, None, None, None
-
-
 def stacked_eligible(layer, x: torch.Tensor) -> bool:
     """Grouped (one group per stacked pair) implicit-GEMM path of ``sim/stacked.py::StackedConv2d``: all three directions on the
     TMA-im2col GEMM kernels, which needs 64-channel chunks on both sides."""
@@ -290,31 +251,15 @@ class TcConv2d(nn.Module):
             bound = 1 / math.sqrt(fan_in) if fan_in > 0 else 0
             nn.init.uniform_(self.bias, -bound, bound)
 
-    def _eligible(self, x: torch.Tensor) -> bool:
-        k = self.weight[0].numel()
-        return (x.is_cuda and x.dim() == 4 and self.groups == 1 and self.dilation == (1, 1) and k % 8 == 0 and k >= 64
-                and self.out_channels % 8 == 0 and self.out_channels >= 16 and _ext.available())
-
     def _use_igemm(self, x: torch.Tensor) -> bool:
-        if not (x.is_cuda and x.dim() == 4 and _ext.available() and os.environ.get("FDB_CONV_IM2COL") != "1"
-                and os.environ.get("FDB_NO_TC_CONV") != "1" and hasattr(_ext.load(), "conv_igemm_fwd")
-                and igemm_eligible(self.in_channels, self.out_channels, self.stride, self.dilation, self.groups)):
-            return False
-        # FDB_CONV_POLICY: "igemm" = every eligible layer on the hand-written kernels (default); "auto" = leave layers with fewer
-        # than 2048 output pixels that only the gather kernels cover to the library (a 128-pixel-row tile grid cannot fill 132
-        # SMs there)
-        if os.environ.get("FDB_CONV_POLICY", "igemm") == "auto" and not tma_eligible(self.in_channels, self.stride, self.padding, self.kernel_size):
-            ho = (x.shape[2] + 2 * self.padding[0] - self.kernel_size[0]) // self.stride[0] + 1
-            wo = (x.shape[3] + 2 * self.padding[1] - self.kernel_size[1]) // self.stride[1] + 1
-            return x.shape[0] * ho * wo >= 2048
-        return True
+        return (x.is_cuda and x.dim() == 4 and _ext.available() and os.environ.get("FDB_NO_TC_CONV") != "1"
+                and hasattr(_ext.load(), "conv_igemm_fwd")
+                and igemm_eligible(self.in_channels, self.out_channels, self.stride, self.dilation, self.groups))
 
     def forward(self, x):
         relu = self.activation == "relu"
         if self._use_igemm(x):
             return _ConvIgemmFn.apply(x, self.weight, self.bias, self.stride, self.padding, relu)
-        if self._eligible(x) and os.environ.get("FDB_CONV_IM2COL") == "1":
-            return _TcConvFn.apply(x, self.weight, self.bias, self.stride, self.padding, relu)
         w = self.weight
         if not x.is_cuda:       # CPU: canonical (contiguous NCHW) formats only — see models.utils.unflatten_to_state_dict
             x, w = x.contiguous(), w.contiguous()

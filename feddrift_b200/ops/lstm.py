@@ -74,10 +74,10 @@ class Lstm2Workspace:
 
 
 def lstm2_pairs_forward(arena: torch.Tensor, row_off: torch.Tensor, offs: Sequence[int], tokens: torch.Tensor, E: int,
-                        ws: Lstm2Workspace, dbg: Optional[torch.Tensor] = None) -> None:
+                        ws: Lstm2Workspace) -> None:
     """tokens: int32 ``[npairs, 16, T]``; row_off: int64 ``[npairs]`` element offsets of the pairs' parameter rows in ``arena``."""
     CALLS["fwd"] += 1
-    _ext.load(required=True).lstm2_forward(arena, row_off, [int(o) for o in offs], tokens, ws.gates, ws.cst, ws.hhist, ws.hlast, int(E), dbg)
+    _ext.load(required=True).lstm2_forward(arena, row_off, [int(o) for o in offs], tokens, ws.gates, ws.cst, ws.hhist, ws.hlast, int(E))
 
 
 def lstm2_pairs_backward(arena: torch.Tensor, row_off: torch.Tensor, offs: Sequence[int], tokens: torch.Tensor, E: int,

@@ -175,16 +175,6 @@ def _peer_aggregate(sim, world, rank):
         sim.bank.theta.copy_(pa.theta)
 
 
-def _nhwc(x: torch.Tensor) -> torch.Tensor:
-    """Opt-in (``FDB_NHWC=1``) channels_last activations for conv nets.  With NCHW activations the library spends part of a
-    ResNet-18 step in nchwToNhwc / nhwcToNchw conversion kernels (tools/profile_generic.py shows how much); NHWC kernels need
-    16-byte aligned weight pointers (the arena aligns every big tensor, models/utils.py::flat_spec).  The NHWC path has not
-    been validated end to end, so it stays opt-in."""
-    if os.environ.get("FDB_NHWC") == "1" and x.is_cuda and x.dim() == 4:
-        return x.contiguous(memory_format=torch.channels_last)
-    return x
-
-
 def _lazy_client_xy(Xc_all, data, c, T1, S):
     cache = []
 
@@ -254,7 +244,7 @@ class _GraphedStep:
             else:
                 x, y = self.x, self.y
             self.g.zero_()
-            F.cross_entropy(self.mod(_nhwc(x)), y).backward()
+            F.cross_entropy(self.mod(x), y).backward()
             if self.use_adam:
                 ops.adam_amsgrad_rows_(self.row.view(1, -1), self.g.view(1, -1), self.m.view(1, -1), self.v.view(1, -1),
                                        self.vmax.view(1, -1), self.step, self.lr, self.wd)
@@ -394,7 +384,7 @@ def _local_steps(sim, c, m, xy, sampler, seed, rnd, E, use_adam, lr, wd, feat_ma
         else:
             for p_ in mod.parameters():
                 p_.grad = None
-            F.cross_entropy(mod(_nhwc(xb)), yb).backward()
+            F.cross_entropy(mod(xb), yb).backward()
             g = _flat_grads(mod, bank, row)
         r2 = row.reshape(1, -1)
         if use_adam:

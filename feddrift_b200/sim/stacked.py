@@ -35,8 +35,6 @@ from .. import ops
 from ..models.utils import ohwi_stored
 from ..ops.reference import batch_hash, mix32
 
-_GRAPH_DEFAULT = "0"      # FDB_STACKED_GRAPH: capture the stacked E-step training as one CUDA graph
-
 _PASS = (nn.ReLU, nn.MaxPool2d, nn.AvgPool2d, nn.AdaptiveAvgPool2d, nn.Dropout, nn.Dropout2d, nn.Flatten, nn.Identity)
 
 
@@ -130,8 +128,8 @@ class StackedBatchNorm2d(_Stacked):
         if self.training:
             self.steps += 1
         mom = self.momentum if self.momentum is not None else 0.1
-        if (self.training and x.is_cuda and x.dim() == 4 and self.weight is not None and os.environ.get("FDB_NO_BN_KERNEL") != "1"
-                and ops.native(x) and hasattr(ops._ext.load(), "bn_nhwc_fwd")):
+        if (self.training and x.is_cuda and x.dim() == 4 and self.weight is not None and ops.native(x)
+                and hasattr(ops._ext.load(), "bn_nhwc_fwd")):
             # npairs·C channels, few rows: the coalesced NHWC kernels (csrc/misc.cu)
             return ops.batch_norm_train_nhwc(x, self.weight, self.bias, self.running_mean if self.track else None,
                                              self.running_var if self.track else None, self.eps, mom)
@@ -290,8 +288,7 @@ class _Stage:
                 getattr(bn, attr).copy_(self.params[:, off:off + C].reshape(-1))
             bn.steps = 0
 
-    def store_buffers(self, steps: Optional[int] = None) -> None:
-        """``steps``: BatchNorm forward passes of this round (a replayed CUDA graph does not run the Python counter)."""
+    def store_buffers(self) -> None:
         for name, bn in self.bns:
             C = bn.num_features
             for attr in ("running_mean", "running_var"):
@@ -299,7 +296,7 @@ class _Stage:
                 self.params[:, off:off + C].copy_(getattr(bn, attr).view(self.npairs, C))
             key = f"{name}.num_batches_tracked"
             if key in self.spec:
-                self.params[:, self.spec[key][1]] += float(bn.steps if steps is None else steps)
+                self.params[:, self.spec[key][1]] += float(bn.steps)
 
 
 def max_pairs_per_pass(P: int) -> int:
@@ -367,63 +364,20 @@ def _train_pass(sim, pairs: List, seed: int, rnd: int, E: int, use_adam: bool, l
     Yf = sim.data.Y.reshape(-1)
     tmpl = bank.template
 
-    def steps(idx: torch.Tensor) -> None:
-        for e in range(E):
-            x = Xf[idx[e]]                                                    # [npairs, B, *features]
-            y = Yf[idx[e]].long()                                             # [npairs, B]
-            st.grads.zero_()
-            logits = st.net(stack_input(tmpl, x))                             # [B, npairs·K]
-            K = logits.shape[1] // npairs
-            # Σ_pairs mean_B CE: every pair's gradient is exactly its own mean-reduced loss gradient
-            loss = F.cross_entropy(logits.reshape(B * npairs, K), y.t().reshape(-1), reduction="sum") / B
-            loss.backward()
-            if use_adam:
-                ops.adam_amsgrad_rows_(st.params, st.grads, st.m, st.v, st.vmax, st.step, lr, wd)
-            else:
-                ops.sgd_rows_(st.params, st.grads, lr, 0.0)
-
-    # The whole E-step training of all pairs as ONE CUDA graph over the staged rows (the eager stacked step is ≈ 400 launches
-    # for a ResNet-18 and host-bound).  First call with a given shape runs eagerly (warm-up: lazy inits, autotuning), the
-    # second captures, later ones replay; any capture failure falls back to eager execution for good.
-    key = (npairs, B, E, bool(use_adam), float(lr), float(wd), tuple(gidx.shape))
-    use_graph = (dev.type == "cuda" and os.environ.get("FDB_STACKED_GRAPH", _GRAPH_DEFAULT) == "1" and os.environ.get("FDB_NO_GRAPHS") != "1"
-                 and not sim.__dict__.get("_stack_graph_broken", False))
-    g = st.__dict__.get("graph") if use_graph else None
-    if g is not None and g["key"] == key:
-        g["idx"].copy_(gidx, non_blocking=True)
-        g["graph"].replay()
-    elif use_graph and st.__dict__.get("warm_key") == key:
-        st.captures = st.__dict__.get("captures", 0) + 1
-        if st.captures > 4:                        # e.g. Adaptive-FedAvg changes lr every round: re-capturing would cost more than it saves
-            sim._stack_graph_broken = True
-        try:
-            idx_static = gidx.clone()
-            cs = torch.cuda.Stream(device=dev)
-            cs.wait_stream(torch.cuda.current_stream(dev))
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph, stream=cs):
-                steps(idx_static)
-            torch.cuda.current_stream(dev).wait_stream(cs)
-            st.graph = {"key": key, "graph": graph, "idx": idx_static, "stream": cs}
-            graph.replay()
-        except Exception as exc:  # noqa: BLE001  (capture is an optimisation; the eager path is always valid)
-            import logging
-            logging.warning("CUDA-graph capture of the stacked step failed (%s); running eagerly", exc)
-            sim._stack_graph_broken = True
-            torch.cuda.synchronize()
-            st.load_buffers()                      # a failed capture executed nothing: restart this round's steps eagerly
-            torch.index_select(bank.theta, 0, ms, out=st.params)
-            if use_adam:
-                torch.index_select(cl.m.view(CM, P), 0, rows, out=st.m)
-                torch.index_select(cl.v.view(CM, P), 0, rows, out=st.v)
-                torch.index_select(cl.vmax.view(CM, P), 0, rows, out=st.vmax)
-                st.step.copy_(cl.step.view(-1).index_select(0, rows))
-            steps(gidx)
-    else:
-        st.warm_key = key
-        st.graph = None
-        steps(gidx)
-    st.store_buffers(E)
+    for e in range(E):
+        x = Xf[gidx[e]]                                                       # [npairs, B, *features]
+        y = Yf[gidx[e]].long()                                                # [npairs, B]
+        st.grads.zero_()
+        logits = st.net(stack_input(tmpl, x))                                 # [B, npairs·K]
+        K = logits.shape[1] // npairs
+        # Σ_pairs mean_B CE: every pair's gradient is exactly its own mean-reduced loss gradient
+        loss = F.cross_entropy(logits.reshape(B * npairs, K), y.t().reshape(-1), reduction="sum") / B
+        loss.backward()
+        if use_adam:
+            ops.adam_amsgrad_rows_(st.params, st.grads, st.m, st.v, st.vmax, st.step, lr, wd)
+        else:
+            ops.sgd_rows_(st.params, st.grads, lr, 0.0)
+    st.store_buffers()
     cl.params.view(CM, P).index_copy_(0, rows, st.params)
     if use_adam:
         cl.m.view(CM, P).index_copy_(0, rows, st.m)

@@ -1,5 +1,5 @@
-"""Pair-stacked executor on the GPU: the CUDA-graph replay of the stacked E-step training equals its eager execution, and
-the stacked path equals the per-pair path (SGD, dropout-free CNN; see tests/test_stacked.py for the CPU equivalence proofs)."""
+"""Pair-stacked executor on the GPU: the stacked path equals the per-pair path (SGD, dropout-free CNN; see tests/test_stacked.py
+for the CPU equivalence proofs)."""
 import os
 
 import pytest
@@ -8,10 +8,10 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-def _run(stacked: str, graph: str, rounds: int = 3):
+def _run(stacked: str, rounds: int = 3):
     from feddrift_b200.sim import DriftSim, make_args
     from feddrift_b200.utils.metrics import MetricsSink
-    os.environ["FDB_STACKED"], os.environ["FDB_STACKED_GRAPH"] = stacked, graph
+    os.environ["FDB_STACKED"] = stacked
     try:
         a = make_args(model="cnn", dataset="MNIST", client_num_in_total=6, client_num_per_round=6, concept_drift_algo="win-1",
                       concept_drift_algo_arg="", concept_num=2, change_points="A", sample_num=16, batch_size=8, comm_round=rounds,
@@ -21,19 +21,13 @@ def _run(stacked: str, graph: str, rounds: int = 3):
             mod.p = 0.0
         sim.run_time_step(0, rounds=rounds)
         torch.cuda.synchronize()
-        st = sim.__dict__.get("_stack_stage")
-        return sim.bank.theta.clone(), (st is not None and st.__dict__.get("graph") is not None), bool(sim.__dict__.get("_stack_graph_broken", False))
+        return sim.bank.theta.clone()
     finally:
         os.environ.pop("FDB_STACKED", None)
-        os.environ.pop("FDB_STACKED_GRAPH", None)
 
 
-def test_stacked_graph_replay_equals_eager_and_per_pair():
-    th_graph, graphed, broken = _run("force", "1")
-    assert graphed and not broken                     # round 1 eager warm-up, round 2 capture + replay, round 3 replay
-    th_eager, g2, _ = _run("force", "0")
-    assert not g2
-    th_pair, _, _ = _run("0", "0")
+def test_stacked_equals_per_pair():
+    th_stacked = _run("force")
+    th_pair = _run("0")
     scale = th_pair.abs().max().item()
-    assert (th_graph - th_eager).abs().max().item() < 2e-3 * scale
-    assert (th_eager - th_pair).abs().max().item() < 2e-2 * scale      # bf16 tensor-core operands on both sides, different summation orders
+    assert (th_stacked - th_pair).abs().max().item() < 2e-2 * scale     # bf16 tensor-core operands on both sides, different summation orders

@@ -41,19 +41,6 @@ if len(sys.argv) > 2 and sys.argv[1] == "--once":
     torch.cuda.synchronize()
     sys.exit(0)
 
-if len(sys.argv) > 2 and sys.argv[1] == "--segments":   # SM-clock cycles per segment of the forward phase loop
-    for n in [int(v) for v in sys.argv[2:]]:
-        arena, row_off, tok, ws, dh = setup(n)
-        dbg = torch.zeros(8, dtype=torch.int64, device=dev)
-        for _ in range(3):
-            L.lstm2_pairs_forward(arena, row_off, offs, tok, 8, ws, dbg)
-        torch.cuda.synchronize()
-        names = ["issuer:wait_inbound", "issuer:mma_issue", "L1grp:wait_mma", "L1grp:epilogue+bar", "L1grp:cell+stage+bar", "L1grp:bulk_issue", "-", "-"]
-        v = dbg.tolist()
-        print(json.dumps({"clusters": n, "phases": T + 1, "cycles_per_phase": {k: round(x / (T + 1)) for k, x in zip(names, v)},
-                          "total_per_phase": round(sum(v) / (T + 1))}))
-    sys.exit(0)
-
 clk = ClockSampler(0)
 clk.start()
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
