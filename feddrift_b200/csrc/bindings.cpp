@@ -27,7 +27,8 @@ std::vector<int64_t> fed_round_small(
     c10::optional<Tensor> eval_train_model, c10::optional<Tensor> eval_test_model, c10::optional<Tensor> ens_w,
     c10::optional<Tensor> client_out, c10::optional<Tensor> lr_dev, Tensor metrics, c10::optional<Tensor> timers,
     std::vector<double> fcfg, std::vector<int64_t> icfg, std::vector<int64_t> peer_inbox,
-    c10::optional<Tensor> error_flag, c10::optional<Tensor> counters, std::vector<int64_t> peer_metrics, std::vector<int64_t> host_io) {
+    c10::optional<Tensor> error_flag, c10::optional<Tensor> counters, std::vector<int64_t> peer_metrics, std::vector<int64_t> host_io,
+    c10::optional<Tensor> participation) {
     CHECK_CUDA_F32(X); CHECK_CUDA_I32(Y); CHECK_CUDA_I32(nsamp); CHECK_CUDA_F32(W); CHECK_CUDA_F32(theta); CHECK_CUDA_I32(opt_step);
     CHECK_CUDA_F32(metrics);
     TORCH_CHECK(X.is_contiguous() && Y.is_contiguous() && nsamp.is_contiguous() && W.is_contiguous() && metrics.is_contiguous(),
@@ -81,6 +82,15 @@ std::vector<int64_t> fed_round_small(
     if (p.world > 1 && (int)peer_metrics.size() == p.world)
         for (int g = 0; g < p.world; ++g) p.metrics_peer[g] = reinterpret_cast<float*>(peer_metrics[g]);
     if (p.use_adam) TORCH_CHECK(p.opt_m && p.opt_v && p.opt_vmax, "adam needs optimizer state tensors");
+    if (participation.has_value() && participation->defined()) {   // [rows, C] uint8: row (round % rows) lists who trains
+        const Tensor& pt = *participation;
+        TORCH_CHECK(pt.is_cuda() && pt.device() == X.device() && pt.scalar_type() == torch::kUInt8,
+                    "fed_round_small: participation must be a uint8 tensor on the device of X");
+        TORCH_CHECK(pt.is_contiguous() && pt.dim() == 2 && pt.size(0) >= 1 && pt.size(1) == p.C,
+                    "fed_round_small: participation must be contiguous [rows >= 1, C]");
+        p.part = pt.data_ptr<uint8_t>();
+        p.part_rows = (int)pt.size(0);
+    }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
     TORCH_CHECK(rc != -1, "fed_round_small: MLP shape (", kind, ",", din, ",", hid, ",", dout, ") is not instantiated");

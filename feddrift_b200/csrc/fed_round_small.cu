@@ -186,7 +186,10 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
         const int buf = r & 1;
 
         // ------------------------------------------------------------------ prep: pair list from W
+        // Partial participation: only the clients of this round's table row train and enter the cluster totals, so the
+        // prep runs every round.  The row follows the device round counter (graph replay picks the right one).
         if (need_prep) {
+            const unsigned char* prow = p.part ? p.part + (size_t)(rnd % (unsigned)p.part_rows) * C : nullptr;
             for (int k = tid; k < CM; k += blockDim.x) {
                 const int c = k / M, m = k % M;
                 float n = 0.f;
@@ -220,7 +223,7 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     for (int c = 0; c < C; ++c) act |= (p.W[(t * M + m) * C + c] != 0.f);
                 }
                 float tot = 0.f;
-                if (act) for (int c = 0; c < C; ++c) tot += ncm_s[c * M + m];
+                if (act) for (int c = 0; c < C; ++c) if (!prow || prow[c]) tot += ncm_s[c * M + m];
                 active_s[m] = act;
                 tot_s[m] = tot;
             }
@@ -232,7 +235,7 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     bool on = false;
                     if (k < CM) {
                         const int c = k / M, m = k % M;
-                        on = active_s[m] && ncm_s[k] > 0.f && (p.world == 1 || (c % p.world) == p.rank);
+                        on = active_s[m] && ncm_s[k] > 0.f && (!prow || prow[c]) && (p.world == 1 || (c % p.world) == p.rank);
                     }
                     const unsigned mask = __ballot_sync(0xffffffffu, on);
                     if (on) pairs_s[base + __popc(mask & ((1u << lane) - 1u))] = k;
@@ -241,7 +244,7 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                 if (lane == 0) misc_s[0] = base;
             }
             __syncthreads();
-            need_prep = (p.recluster_hard != 0);
+            need_prep = (p.recluster_hard != 0) || (p.part != nullptr);
         }
         const int npairs = misc_s[0];
 

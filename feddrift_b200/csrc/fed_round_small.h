@@ -19,6 +19,8 @@ struct RoundParams {
     const int* eval_train_model;  // [C] or nullptr (-1 → argmax_m W[t, m, c])
     const int* eval_test_model;   // [C] or nullptr
     const float* ens_w;        // [C, M] or nullptr
+    const unsigned char* part; // [part_rows, C] client participation (row = round % part_rows) or nullptr: everyone trains
+    int part_rows;
     // model / optimizer state
     float* theta;        // [M, theta_stride]
     float* opt_m;        // [C, M, P]

@@ -190,6 +190,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     Optional: ``feat_mask [M,din]`` (training inputs only, KUE), ``recluster_hard`` (IFCA per-round argmax
     re-clustering), ``eval_train_model``/``eval_test_model`` [C] int (-1 → argmax_m W[t,m,c]),
     ``ens_mode`` 0|1 (weighted hard vote)|2 (weighted soft vote) with ``ens_w [C,M]`` for the TEST metric.
+    ``participation [rows, C]`` bool/uint8: in round ``rnd`` only the clients of row ``rnd % rows`` train and enter the
+    cluster averages (a cluster with no participant keeps its model); evaluation and re-clustering still cover every client.
     Mutates theta / opt state / W (if recluster) in place; returns ``metrics [rounds, C, 4]`` =
     (train_correct, train_loss_sum, test_correct, test_loss_sum) and ``counts [C, 2]`` = (n_train, n_test).
     """
@@ -206,8 +208,12 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     feat_mask = st.get("feat_mask")
     ens_mode = int(st.get("ens_mode", 0) or 0)
     Xflat = X.reshape(T1, C, S, -1)
+    part = st.get("participation")
+    if part is not None:
+        part = torch.as_tensor(part).to("cpu", torch.bool)
     for r in range(rounds):
         rnd = round0 + r
+        prow = part[rnd % part.shape[0]] if part is not None else None
         cur_lr = float(st["lr"])
         Wt = W[t]
         if st.get("sample_mode", "pool") == "index":
@@ -217,6 +223,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
         acc_w = torch.zeros(M, dtype=torch.float64)
         locals_: Dict[Tuple[int, int], Tuple[torch.Tensor, float]] = {}
         for c in range(C):
+            if prow is not None and not bool(prow[c]):
+                continue
             Xc = Xflat[:, c].reshape(T1 * S, -1)
             Yc = Y[:, c].reshape(T1 * S)
             for m in range(M):

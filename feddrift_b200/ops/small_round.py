@@ -63,7 +63,10 @@ def prepare(st: Dict) -> Dict:
         cache["feat_mask"] = _f32(st.get("feat_mask"), dev)
         cache["eval_train_model"] = _i32(st.get("eval_train_model"), dev)
         cache["eval_test_model"] = _i32(st.get("eval_test_model"), dev)
-        # launch shape hints: warps per pair from the mini-batch size, cluster size from the active pair count
+        part = st.get("participation")   # [rows, C] bool/uint8 or None (everyone takes part)
+        cache["participation"] = None if part is None else part.to(device=dev, dtype=torch.uint8).contiguous()
+        # launch shape hints: warps per pair from the mini-batch size, cluster size from the active pair count (counted
+        # as if every client took part: an upper bound when clients are sampled)
         B, t = int(st["batch_size"]), int(st["t_cur"])
         bmax = min(B, int(cache["nsamp"].max()))
         cache["wpp"] = 4 if bmax > 64 else (2 if bmax > 32 else 1)
@@ -129,7 +132,8 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         cache["train_index"], cache["train_count"], cache["feat_mask"], cache["eval_train_model"], cache["eval_test_model"],
         ens_w, st.get("client_out"), lr_dev, metrics_out, st.get("timers"), fcfg, icfg,
         list(mg["inbox_ptrs"]) if mg else [], mg.get("error_flag") if mg else None,
-        st.get("counters"), peer_metrics, [int(v) for v in st["host_io"]] if st.get("host_io") else [])
+        st.get("counters"), peer_metrics, [int(v) for v in st["host_io"]] if st.get("host_io") else [],
+        cache["participation"])
     if mg:
         mg["flag_base"] = int(mg["flag_base"]) + rounds
     if st.get("counters") is not None:

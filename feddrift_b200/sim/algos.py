@@ -550,6 +550,9 @@ class ClusterFLAlgo(DriftAlgo):
         from ..drift.hclust import complete_linkage_bipartition
         self.split_done = True
         members = np.nonzero(self.assign == 0)[0]
+        part = self.sim.participants(self.split_round)
+        if part is not None:   # only clients that trained in the split round uploaded an update; the others stay on model 0
+            members = members[part[members]]
         if len(members) < 2 or self.args.concept_num < 2:
             return False
         U = client_params[members.tolist(), 0, :] - self.sim.bank.theta[0][None, :]

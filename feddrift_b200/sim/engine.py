@@ -38,6 +38,7 @@ from ..models.utils import create_model
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
 from . import checkpoint as ckpt
+from .sampling import sample_clients
 
 DEFAULTS = dict(
     model="fnn", dataset="sea", client_num_in_total=10, client_num_per_round=10, batch_size=500,
@@ -77,6 +78,9 @@ class DriftSim:
         self.data_host = data
         self.data = data.to(self.device)
         self.C = data.client_num
+        self.participation = self._participation_table()
+        self._participation_dev = None if self.participation is None else \
+            torch.from_numpy(self.participation.astype(np.uint8)).to(self.device)
         from .algos import make_algo
         self.algo = algo if algo is not None else make_algo(args, self)
         self.M = self.algo.num_model_slots()
@@ -97,6 +101,27 @@ class DriftSim:
         self.clients = ClientArena(self.C, self.M, self.bank.P, self.device,
                                    adam=(args.client_optimizer != "sgd"))
         self.timings = {"cluster_s": 0.0, "rounds_s": 0.0}
+
+    def _participation_table(self) -> Optional[np.ndarray]:
+        """``[comm_round, C]`` bool table of the clients that train in each round of a time step (``sample_clients``), or
+        None when ``client_num_per_round >= C`` (everyone trains every round)."""
+        K = int(getattr(self.args, "client_num_per_round", self.C))
+        if K < 1:
+            raise ValueError(f"client_num_per_round must be >= 1 (got {K})")
+        if K >= self.C:
+            return None
+        R = max(int(self.args.comm_round), 1)
+        table = np.zeros((R, self.C), dtype=bool)
+        for r in range(R):
+            table[r, sample_clients(r, self.C, K)] = True
+        return table
+
+    def participants(self, rnd: int) -> Optional[np.ndarray]:
+        """Bool ``[C]`` mask of the clients that train in round ``rnd`` of a time step (None: all of them).  A round past
+        ``comm_round`` reuses row ``rnd % comm_round``."""
+        if self.participation is None:
+            return None
+        return self.participation[rnd % self.participation.shape[0]]
 
     # ------------------------------------------------------------------ experiment driver
     def run(self, start_iteration: int = 0, end_iteration: Optional[int] = None) -> Dict:
@@ -169,6 +194,8 @@ class DriftSim:
                     self._small[k] = plan[k]
             if self._small["optimizer"] == "sgd":
                 self._small["wd"] = 0.0
+            if self._participation_dev is not None:
+                self._small["participation"] = self._participation_dev
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)

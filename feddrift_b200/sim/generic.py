@@ -72,8 +72,11 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
         bpairs, n_host = [], np.zeros((C, M), dtype=np.float32)
         slots = [] if batched else _stream_slots(sim)    # K side streams: independent (client, model) pairs replay concurrently
         pair_i = 0
+        prow = sim.participants(rnd)
         for c in range(C):
             if world > 1 and c % world != rank:   # clients are sharded over the ranks (one process per GPU)
+                continue
+            if prow is not None and not prow[c]:   # not sampled this round: no training, weight 0 in the aggregate
                 continue
             xy = _lazy_client_xy(Xc_all, data, c, T1, S)
             for m in range(M):
