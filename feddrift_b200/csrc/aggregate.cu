@@ -30,10 +30,15 @@ static inline size_t smem_floats(int n) { return ((size_t)n + 4) * sizeof(float)
 // ------------------------------------------------------------------------------------------------ K1
 // theta[m, :] = Σ_c (n[c,m]/tot[m]) · cp[c, m, :]   for every m with tot[m] > 0.
 // server_opt != 0 fuses the FedOpt step: g = theta_old - avg, then sgd(+momentum)/adam/adagrad/yogi on theta.
+// steps != nullptr: per-slot step counts [M] (steps already applied; the kernel only reads them, the launcher's caller
+// advances the slots that aggregated), Adam's bias corrections then use t = steps[m] + 1 instead of the launch-wide bc1 / bc2.
+// mask != nullptr: [P] entries with mask[i] == 0 (BatchNorm statistics) take the plain average and keep their state.
 struct ServerOpt {
     int kind;  // 0 none (plain overwrite), 1 sgd, 2 adam, 3 adagrad, 4 yogi
     float lr, momentum, b1, b2, eps, bc1, bc2;
     float *s0, *s1;  // optimizer state rows [M, P] (momentum / m , v)
+    const int* steps;
+    const unsigned char* mask;
 };
 
 __global__ void __launch_bounds__(256) cluster_aggregate_kernel(float* __restrict__ theta, int theta_stride,
@@ -51,6 +56,11 @@ __global__ void __launch_bounds__(256) cluster_aggregate_kernel(float* __restric
         for (int c = threadIdx.x; c < C; c += blockDim.x) wsm[c] = n[c * M + m] / tot;
         __syncthreads();
         float* out = theta + (size_t)m * theta_stride;
+        float bc1 = so.bc1, bc2 = so.bc2;
+        if (so.kind != 0 && so.steps) {
+            const float ts = (float)(so.steps[m] + 1);
+            bc1 = 1.f - powf(so.b1, ts); bc2 = 1.f - powf(so.b2, ts);
+        }
         const size_t cstride = (size_t)M * P;
         const float* base = cp + (size_t)m * P;
         const bool vec_ok = ((P & 3) == 0) && ((((uintptr_t)base) & 15) == 0) && ((((uintptr_t)out) & 15) == 0) && ((cstride & 3) == 0);
@@ -80,31 +90,10 @@ __global__ void __launch_bounds__(256) cluster_aggregate_kernel(float* __restric
                     const float o4[4] = {old.x, old.y, old.z, old.w};
 #pragma unroll
                     for (int u = 0; u < 4; ++u) {
-                        const size_t idx = (size_t)m * P + (size_t)i * 4 + u;
-                        const float g = o4[u] - r[u];
-                        float th = o4[u];
-                        if (so.kind == 1) {
-                            float gg = g;
-                            if (so.momentum != 0.f) { gg = so.s0[idx] * so.momentum + g; so.s0[idx] = gg; }
-                            th -= so.lr * gg;
-                        } else if (so.kind == 2) {
-                            const float mm = so.s0[idx] * so.b1 + (1.f - so.b1) * g;
-                            const float vv = so.s1[idx] * so.b2 + (1.f - so.b2) * g * g;
-                            so.s0[idx] = mm; so.s1[idx] = vv;
-                            th -= (so.lr / so.bc1) * mm / (sqrtf(vv) / sqrtf(so.bc2) + so.eps);
-                        } else if (so.kind == 3) {
-                            const float ss = so.s0[idx] + g * g;
-                            so.s0[idx] = ss;
-                            th -= so.lr * g / (sqrtf(ss) + so.eps);
-                        } else {
-                            const float mm = so.s0[idx] * so.b1 + (1.f - so.b1) * g;
-                            const float g2 = g * g, vo = so.s1[idx];
-                            const float sg = (vo - g2 > 0.f) ? 1.f : ((vo - g2 < 0.f) ? -1.f : 0.f);
-                            const float vv = vo - (1.f - so.b2) * sg * g2;
-                            so.s0[idx] = mm; so.s1[idx] = vv;
-                            th -= so.lr * mm / (sqrtf(vv) + so.eps);
-                        }
-                        r[u] = th;
+                        const size_t i1 = (size_t)i * 4 + u;
+                        if (so.mask && !so.mask[i1]) continue;
+                        r[u] = server_opt_update(so.kind, o4[u], r[u], so.s0, so.s1, (size_t)m * P + i1, so.lr, so.momentum, so.b1,
+                                                 so.b2, so.eps, bc1, bc2);
                     }
                 }
                 reinterpret_cast<float4*>(out)[i] = make_float4(r[0], r[1], r[2], r[3]);
@@ -113,34 +102,9 @@ __global__ void __launch_bounds__(256) cluster_aggregate_kernel(float* __restric
             for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < P; i += gridDim.x * blockDim.x) {
                 float acc = 0.f;
                 for (int c = 0; c < C; ++c) acc = fmaf(base[(size_t)c * cstride + i], wsm[c], acc);
-                if (so.kind == 0) out[i] = acc;
-                else {
-                    const size_t idx = (size_t)m * P + i;
-                    const float g = out[i] - acc;
-                    float th = out[i];
-                    if (so.kind == 1) {
-                        float gg = g;
-                        if (so.momentum != 0.f) { gg = so.s0[idx] * so.momentum + g; so.s0[idx] = gg; }
-                        th -= so.lr * gg;
-                    } else if (so.kind == 2) {
-                        const float mm = so.s0[idx] * so.b1 + (1.f - so.b1) * g;
-                        const float vv = so.s1[idx] * so.b2 + (1.f - so.b2) * g * g;
-                        so.s0[idx] = mm; so.s1[idx] = vv;
-                        th -= (so.lr / so.bc1) * mm / (sqrtf(vv) / sqrtf(so.bc2) + so.eps);
-                    } else if (so.kind == 3) {
-                        const float ss = so.s0[idx] + g * g;
-                        so.s0[idx] = ss;
-                        th -= so.lr * g / (sqrtf(ss) + so.eps);
-                    } else {
-                        const float mm = so.s0[idx] * so.b1 + (1.f - so.b1) * g;
-                        const float g2 = g * g, vo = so.s1[idx];
-                        const float sg = (vo - g2 > 0.f) ? 1.f : ((vo - g2 < 0.f) ? -1.f : 0.f);
-                        const float vv = vo - (1.f - so.b2) * sg * g2;
-                        so.s0[idx] = mm; so.s1[idx] = vv;
-                        th -= so.lr * mm / (sqrtf(vv) + so.eps);
-                    }
-                    out[i] = th;
-                }
+                if (so.kind == 0 || (so.mask && !so.mask[i])) out[i] = acc;
+                else out[i] = server_opt_update(so.kind, out[i], acc, so.s0, so.s1, (size_t)m * P + i, so.lr, so.momentum, so.b1, so.b2,
+                                                so.eps, bc1, bc2);
             }
         }
         __syncthreads();
@@ -149,11 +113,11 @@ __global__ void __launch_bounds__(256) cluster_aggregate_kernel(float* __restric
 
 int cluster_aggregate_launch(float* theta, int theta_stride, const float* cp, const float* n, int C, int M, int P, float* tot_out,
                              int opt_kind, float lr, float momentum, float b1, float b2, float eps, int step, float* s0, float* s1,
-                             cudaStream_t stream) {
+                             const int* steps, const unsigned char* mask, cudaStream_t stream) {
     ServerOpt so{};
     so.kind = opt_kind; so.lr = lr; so.momentum = momentum; so.b1 = b1; so.b2 = b2; so.eps = eps;
     so.bc1 = 1.f - powf(b1, (float)max(step, 1)); so.bc2 = 1.f - powf(b2, (float)max(step, 1));
-    so.s0 = s0; so.s1 = s1;
+    so.s0 = s0; so.s1 = s1; so.steps = steps; so.mask = mask;
     const int threads = 256;
     const int gx = persistent_grid((P + 3) / 4, threads);
     dim3 grid(max(1, gx / max(1, min(M, 8))), min(M, 65535));

@@ -28,7 +28,8 @@ std::vector<int64_t> fed_round_small(
     c10::optional<Tensor> client_out, c10::optional<Tensor> lr_dev, Tensor metrics, c10::optional<Tensor> timers,
     std::vector<double> fcfg, std::vector<int64_t> icfg, std::vector<int64_t> peer_inbox,
     c10::optional<Tensor> error_flag, c10::optional<Tensor> counters, std::vector<int64_t> peer_metrics, std::vector<int64_t> host_io,
-    c10::optional<Tensor> participation) {
+    c10::optional<Tensor> participation, c10::optional<Tensor> server_s0, c10::optional<Tensor> server_s1,
+    c10::optional<Tensor> server_step) {
     CHECK_CUDA_F32(X); CHECK_CUDA_I32(Y); CHECK_CUDA_I32(nsamp); CHECK_CUDA_F32(W); CHECK_CUDA_F32(theta); CHECK_CUDA_I32(opt_step);
     CHECK_CUDA_F32(metrics);
     TORCH_CHECK(X.is_contiguous() && Y.is_contiguous() && nsamp.is_contiguous() && W.is_contiguous() && metrics.is_contiguous(),
@@ -48,10 +49,10 @@ std::vector<int64_t> fed_round_small(
     p.lr_ptr = opt_ptr<float>(lr_dev);
     p.metrics = metrics.data_ptr<float>();
     p.timers = (timers.has_value() && timers->defined()) ? reinterpret_cast<long long*>(timers->data_ptr<int64_t>()) : nullptr;
-    // fcfg: lr, wd, beta1, beta2, eps
+    // fcfg: lr, wd, beta1, beta2, eps [, server_lr, server_momentum, server_eps]
     p.lr = (float)fcfg[0]; p.wd = (float)fcfg[1]; p.beta1 = (float)fcfg[2]; p.beta2 = (float)fcfg[3]; p.eps = (float)fcfg[4];
     // icfg: T1, C, S, M, Lmax, batch, epochs, t_cur, rounds, round0, seed, use_adam, sample_mode, n_mode, recluster, ens_mode,
-    //       skip_aggregate, world, rank, flag_base, cluster, spin_timeout_ms
+    //       skip_aggregate, world, rank, flag_base, cluster, spin_timeout_ms, warps_per_pair [, server optimizer kind]
     p.T1 = (int)icfg[0]; p.C = (int)icfg[1]; p.S = (int)icfg[2]; p.M = (int)icfg[3]; p.Lmax = (int)icfg[4];
     p.theta_stride = (int)theta_stride;
     p.batch_size = (int)icfg[5]; p.epochs = (int)icfg[6]; p.t_cur = (int)icfg[7]; p.rounds = (int)icfg[8]; p.round0 = (int)icfg[9];
@@ -61,6 +62,7 @@ std::vector<int64_t> fed_round_small(
     const int cluster = (int)icfg[20];
     p.spin_timeout_ns = (long long)icfg[21] * 1000000LL;
     p.warps_per_pair = icfg.size() > 22 ? (int)icfg[22] : 1;
+    p.sopt_kind = icfg.size() > 23 ? (int)icfg[23] : 0;
     TORCH_CHECK(p.t_cur < 64, "fed_round_small supports t_cur < 64 time steps (use fed_round_small_fits to route)");
     TORCH_CHECK(p.world >= 1 && p.world <= fdb::kMaxPeers, "world must be in [1, 8]");
     if (p.world > 1) {
@@ -91,6 +93,31 @@ std::vector<int64_t> fed_round_small(
         p.part = pt.data_ptr<uint8_t>();
         p.part_rows = (int)pt.size(0);
     }
+    if (p.sopt_kind != 0) {   // per-slot server optimizer: state [M, P] fp32 rows, step counters [M] int32, all on X's device
+        TORCH_CHECK(p.sopt_kind >= 1 && p.sopt_kind <= 4, "fed_round_small: server optimizer kind must be 1..4 (sgd, adam, adagrad, yogi)");
+        TORCH_CHECK(p.world == 1, "fed_round_small: a server optimizer is single-GPU only");
+        TORCH_CHECK(fcfg.size() >= 8, "fed_round_small: server optimizer needs fcfg {.., server_lr, server_momentum, server_eps}");
+        p.sopt_lr = (float)fcfg[5]; p.sopt_momentum = (float)fcfg[6]; p.sopt_eps = (float)fcfg[7];
+        const int64_t M = p.M, P = theta.size(1);
+        auto check_rows = [&](const c10::optional<Tensor>& t, bool required, const char* name) -> float* {
+            if (!(t.has_value() && t->defined())) {
+                TORCH_CHECK(!required, "fed_round_small: this server optimizer needs ", name);
+                return nullptr;
+            }
+            TORCH_CHECK(t->is_cuda() && t->device() == X.device() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() &&
+                        t->dim() == 2 && t->size(0) == M && t->size(1) == P,
+                        "fed_round_small: ", name, " must be a contiguous float32 [M, P] tensor on the device of X");
+            return t->data_ptr<float>();
+        };
+        p.sopt_s0 = check_rows(server_s0, p.sopt_kind != 1 || p.sopt_momentum != 0.f, "server_s0");
+        p.sopt_s1 = check_rows(server_s1, p.sopt_kind == 2 || p.sopt_kind == 4, "server_s1");
+        TORCH_CHECK(server_step.has_value() && server_step->defined(), "fed_round_small: a server optimizer needs server_step");
+        const Tensor& ss = *server_step;
+        TORCH_CHECK(ss.is_cuda() && ss.device() == X.device() && ss.scalar_type() == torch::kInt32 && ss.is_contiguous() &&
+                    ss.dim() == 1 && ss.size(0) == M,
+                    "fed_round_small: server_step must be a contiguous int32 [M] tensor on the device of X");
+        p.sopt_step = ss.data_ptr<int>();
+    }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
     TORCH_CHECK(rc != -1, "fed_round_small: MLP shape (", kind, ",", din, ",", hid, ",", dout, ") is not instantiated");
@@ -99,8 +126,8 @@ std::vector<int64_t> fed_round_small(
     return {info.cluster, info.threads, info.smem_bytes};
 }
 
-bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur) {
-    return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur) != 0;
+bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur, bool server_opt) {
+    return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt) != 0;
 }
 
 bool fed_round_small_supported(int64_t kind, int64_t din, int64_t hid, int64_t dout) {
@@ -129,7 +156,8 @@ Tensor cluster_aggregate(Tensor theta, Tensor cp, Tensor n) {
     TORCH_CHECK(theta.size(0) == M && theta.size(1) == P && theta.stride(1) == 1, "theta must be [M, P] with unit inner stride");
     auto tot = torch::zeros({M}, theta.options());
     CHECK_OK(fdb::cluster_aggregate_launch(theta.data_ptr<float>(), (int)theta.stride(0), cp.data_ptr<float>(), n.data_ptr<float>(), C, M, P,
-                                           tot.data_ptr<float>(), 0, 0.f, 0.f, 0.9f, 0.999f, 1e-8f, 1, nullptr, nullptr, cur_stream()),
+                                           tot.data_ptr<float>(), 0, 0.f, 0.f, 0.9f, 0.999f, 1e-8f, 1, nullptr, nullptr, nullptr, nullptr,
+                                           cur_stream()),
              "cluster_aggregate");
     return tot;
 }
@@ -142,8 +170,43 @@ Tensor cluster_aggregate_opt(Tensor theta, Tensor cp, Tensor n, int64_t opt_kind
     auto tot = torch::zeros({M}, theta.options());
     CHECK_OK(fdb::cluster_aggregate_launch(theta.data_ptr<float>(), (int)theta.stride(0), cp.data_ptr<float>(), n.data_ptr<float>(), C, M, P,
                                            tot.data_ptr<float>(), (int)opt_kind, (float)lr, (float)momentum, (float)b1, (float)b2, (float)eps,
-                                           (int)step, opt_ptr<float>(s0), opt_ptr<float>(s1), cur_stream()),
+                                           (int)step, opt_ptr<float>(s0), opt_ptr<float>(s1), nullptr, nullptr, cur_stream()),
              "cluster_aggregate_opt");
+    return tot;
+}
+
+// K1 + per-slot server optimizer: every slot with total weight > 0 steps with its own counter (bias correction t = steps[m] + 1),
+// then its counter advances; mask [P] uint8 (optional) keeps entries with mask == 0 at the plain average, outside the optimizer.
+Tensor cluster_aggregate_slots(Tensor theta, Tensor cp, Tensor n, int64_t opt_kind, double lr, double momentum, double b1, double b2,
+                               double eps, c10::optional<Tensor> s0, c10::optional<Tensor> s1, Tensor steps, c10::optional<Tensor> mask) {
+    CHECK_CUDA_F32(theta); CHECK_CUDA_F32(cp); CHECK_CUDA_F32(n); CHECK_CUDA_I32(steps);
+    c10::cuda::CUDAGuard guard(theta.device());
+    const int C = (int)cp.size(0), M = (int)cp.size(1), P = (int)cp.size(2);
+    TORCH_CHECK(opt_kind >= 1 && opt_kind <= 4, "cluster_aggregate_slots: kind must be 1..4 (sgd, adam, adagrad, yogi)");
+    TORCH_CHECK(cp.is_contiguous() && n.is_contiguous() && n.numel() == (int64_t)C * M, "cluster_aggregate_slots: cp [C, M, P] and n [C, M] must be contiguous");
+    TORCH_CHECK(theta.size(0) == M && theta.size(1) == P && theta.stride(1) == 1, "theta must be [M, P] with unit inner stride");
+    TORCH_CHECK(steps.is_contiguous() && steps.numel() == M && steps.device() == theta.device(), "cluster_aggregate_slots: steps must be int32 [M]");
+    for (const auto* t : {&s0, &s1}) {
+        if (t->has_value() && (*t)->defined()) {
+            CHECK_CUDA_F32(**t);
+            TORCH_CHECK((*t)->is_contiguous() && (*t)->dim() == 2 && (*t)->size(0) == M && (*t)->size(1) == P && (*t)->device() == theta.device(),
+                        "cluster_aggregate_slots: optimizer state must be contiguous [M, P] on the device of theta");
+        }
+    }
+    TORCH_CHECK(opt_ptr<float>(s0) || (opt_kind == 1 && momentum == 0.0), "cluster_aggregate_slots: this optimizer needs s0");
+    TORCH_CHECK(opt_ptr<float>(s1) || opt_kind == 1 || opt_kind == 3, "cluster_aggregate_slots: this optimizer needs s1");
+    const unsigned char* mptr = nullptr;
+    if (mask.has_value() && mask->defined()) {
+        TORCH_CHECK(mask->is_cuda() && mask->device() == theta.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                    mask->numel() == P, "cluster_aggregate_slots: mask must be a contiguous uint8 [P] tensor on the device of theta");
+        mptr = mask->data_ptr<uint8_t>();
+    }
+    auto tot = torch::zeros({M}, theta.options());
+    CHECK_OK(fdb::cluster_aggregate_launch(theta.data_ptr<float>(), (int)theta.stride(0), cp.data_ptr<float>(), n.data_ptr<float>(), C, M, P,
+                                           tot.data_ptr<float>(), (int)opt_kind, (float)lr, (float)momentum, (float)b1, (float)b2, (float)eps,
+                                           1, opt_ptr<float>(s0), opt_ptr<float>(s1), steps.data_ptr<int>(), mptr, cur_stream()),
+             "cluster_aggregate_slots");
+    steps.add_((tot > 0).to(torch::kInt32));   // after the launch (same stream): no block reads a counter this launch advances
     return tot;
 }
 
@@ -781,6 +844,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("mlp_eval_matrix", &mlp_eval_matrix);
     m.def("cluster_aggregate", &cluster_aggregate);
     m.def("cluster_aggregate_opt", &cluster_aggregate_opt);
+    m.def("cluster_aggregate_slots", &cluster_aggregate_slots);
     m.def("weighted_average", &weighted_average);
     m.def("fedavg_reduce_apply_peer", &fedavg_reduce_apply_peer);
     m.def("merge_axpby", &merge_axpby);

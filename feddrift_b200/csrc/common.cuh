@@ -109,4 +109,36 @@ struct SpinGuard {
     }
 };
 
+// ---------------------------------------------------------------- FedOpt server step (K11), one entry
+// g = th - avg is the pseudo-gradient; returns the stepped entry.  kind 1 sgd (+momentum), 2 adam, 3 adagrad, 4 yogi;
+// s0[idx] / s1[idx] are the entry's state (sgd: momentum buffer, adagrad: sum of squares, adam / yogi: first / second
+// moment) and are only touched by the kinds that own them; bc1 = 1 - β1^t, bc2 = 1 - β2^t are Adam's bias corrections.
+// Same update law as ops.reference.server_opt_step_.
+FDB_DEVICE float server_opt_update(int kind, float th, float avg, float* s0, float* s1, size_t idx, float lr, float momentum,
+                                   float b1, float b2, float eps, float bc1, float bc2) {
+    const float g = th - avg;
+    if (kind == 1) {
+        float gg = g;
+        if (momentum != 0.f) { gg = s0[idx] * momentum + g; s0[idx] = gg; }
+        th -= lr * gg;
+    } else if (kind == 2) {
+        const float mm = s0[idx] * b1 + (1.f - b1) * g;
+        const float vv = s1[idx] * b2 + (1.f - b2) * g * g;
+        s0[idx] = mm; s1[idx] = vv;
+        th -= (lr / bc1) * mm / (sqrtf(vv) / sqrtf(bc2) + eps);
+    } else if (kind == 3) {
+        const float ss = s0[idx] + g * g;
+        s0[idx] = ss;
+        th -= lr * g / (sqrtf(ss) + eps);
+    } else {
+        const float mm = s0[idx] * b1 + (1.f - b1) * g;
+        const float g2 = g * g, vo = s1[idx];
+        const float sg = (vo - g2 > 0.f) ? 1.f : ((vo - g2 < 0.f) ? -1.f : 0.f);
+        const float vv = vo - (1.f - b2) * sg * g2;
+        s0[idx] = mm; s1[idx] = vv;
+        th -= lr * mm / (sqrtf(vv) + eps);
+    }
+    return th;
+}
+
 }  // namespace fdb

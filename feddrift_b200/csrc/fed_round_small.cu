@@ -41,13 +41,14 @@ struct SmallCfg {
 };
 
 constexpr int kTmax = 64;  // the fused kernel supports t_cur < kTmax time steps (host falls back otherwise)
+constexpr float kServerB1 = 0.9f, kServerB2 = 0.999f;   // server Adam / Yogi betas (ops/server_opt.py)
 
 struct SmemLayout {
-    int theta, part, slot, slot_model, gbuf, thl, wsum, ptab_nb, ptab_w, ncm, tot, active, pairs, misc, total;
+    int theta, part, slot, slot_model, gbuf, thl, wsum, ptab_nb, ptab_w, ncm, tot, active, pairs, misc, sopt, sstep, total;
 };
 
 template <class Net>
-__host__ __device__ inline SmemLayout make_layout(int M, int C, int pairs_per_cta) {
+__host__ __device__ inline SmemLayout make_layout(int M, int C, int pairs_per_cta, bool server_opt) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P;
     SmemLayout L;
@@ -67,6 +68,8 @@ __host__ __device__ inline SmemLayout make_layout(int M, int C, int pairs_per_ct
     L.active = take(M);
     L.pairs = take(C * M);
     L.misc = take(8);
+    L.sopt = take(server_opt ? 2 * M * P : 0);   // server optimizer state [2, M, P], replicated in every CTA like θ
+    L.sstep = take(server_opt ? M : 0);
     L.total = o;
     return L;
 }
@@ -98,7 +101,7 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
     const int C = p.C, M = p.M, S = p.S, t = p.t_cur, B = p.batch_size;
     const int CM = C * M, MP = M * P;
     const int pairs_per_cta = (CM + G - 1) / G;
-    const SmemLayout L = make_layout<Net>(M, C, pairs_per_cta);
+    const SmemLayout L = make_layout<Net>(M, C, pairs_per_cta, p.sopt_kind != 0);
     float* theta_s = smem + L.theta;
     float* part_s = smem + L.part;
     float* slot_s = smem + L.slot;
@@ -116,6 +119,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
     int* active_s = reinterpret_cast<int*>(smem + L.active);
     int* pairs_s = reinterpret_cast<int*>(smem + L.pairs);
     int* misc_s = reinterpret_cast<int*>(smem + L.misc);  // [0] = npairs
+    float* sopt_s = smem + L.sopt;
+    int* sstep_s = reinterpret_cast<int*>(smem + L.sstep);
 
     if (p.host_x != nullptr) {
         // ---- fused H2D: this round's inputs come straight from pinned host memory (each CTA copies 1/G of the range)
@@ -173,6 +178,13 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
     }
     // ---- load the cluster models once (broadcast == this smem fill; afterwards θ never leaves the SM) ----
     for (int e = tid; e < MP; e += blockDim.x) theta_s[e] = p.theta[(e / P) * p.theta_stride + (e % P)];
+    if (p.sopt_kind) {   // server optimizer state: every CTA steps its replica identically (same sums, same order)
+        for (int e = tid; e < MP; e += blockDim.x) {
+            sopt_s[e] = p.sopt_s0 ? p.sopt_s0[e] : 0.f;
+            sopt_s[MP + e] = p.sopt_s1 ? p.sopt_s1[e] : 0.f;
+        }
+        for (int m = tid; m < M; m += blockDim.x) sstep_s[m] = p.sopt_step[m];
+    }
     const float lr = p.lr_ptr ? *p.lr_ptr : p.lr;
     // graph-replay friendly: the round number (RNG stream) and the cross-GPU epoch come from device counters
     const int round0 = p.counters ? p.counters[0] : p.round0;
@@ -435,11 +447,20 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     if (tot_s[m] > 0.f) {
                         float v = 0.f;
                         for (int rk = 0; rk < G; ++rk) v += *(cluster.map_shared_rank(part_s + buf * MP + e, rk));
+                        if (p.sopt_kind) {
+                            const float ts = (float)(sstep_s[m] + 1);
+                            v = server_opt_update(p.sopt_kind, theta_s[e], v, sopt_s, sopt_s + MP, (size_t)e, p.sopt_lr,
+                                                  p.sopt_momentum, kServerB1, kServerB2, p.sopt_eps, 1.f - powf(kServerB1, ts),
+                                                  1.f - powf(kServerB2, ts));
+                        }
                         theta_s[e] = v;
                     }
                 }
             }
             __syncthreads();
+            // every reader of this round's counters is behind the barrier above; the next reads follow the post-training barrier
+            if (p.sopt_kind && p.world == 1)
+                for (int m = tid; m < M; m += blockDim.x) if (tot_s[m] > 0.f) ++sstep_s[m];
         }
         if (p.world > 1) {
             // ---- cross-GPU exchange, LL protocol (flag-in-data, like NCCL's LL): every 8-byte inbox word is
@@ -627,8 +648,16 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
     if (p.counters && crank == 0 && tid == 0) { p.counters[0] = round0 + p.rounds; p.counters[1] = (int)(flag_base + (unsigned)p.rounds); }
     // ---- write the models back (all CTAs hold identical copies; cluster rank 0 stores) ----
     __syncthreads();
-    if (crank == 0)
+    if (crank == 0) {
         for (int e = tid; e < MP; e += blockDim.x) p.theta[(e / P) * p.theta_stride + (e % P)] = theta_s[e];
+        if (p.sopt_kind) {
+            for (int e = tid; e < MP; e += blockDim.x) {
+                if (p.sopt_s0) p.sopt_s0[e] = sopt_s[e];
+                if (p.sopt_s1) p.sopt_s1[e] = sopt_s[MP + e];
+            }
+            for (int m = tid; m < M; m += blockDim.x) p.sopt_step[m] = sstep_s[m];
+        }
+    }
     if (G > 1) cluster.sync();  // keep every CTA's smem alive until all DSMEM reads are done
 }
 
@@ -684,7 +713,7 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     }
     if (G > 8) G = 8;
     const int pairs_per_cta = (CM + G - 1) / G;
-    const SmemLayout L = make_layout<Net>(p.M, p.C, pairs_per_cta);
+    const SmemLayout L = make_layout<Net>(p.M, p.C, pairs_per_cta, p.sopt_kind != 0);
     const int smem = L.total * (int)sizeof(float);
     if (smem > 227 * 1024) return -2;
     auto kern = fed_round_small_kernel<Net>;
@@ -717,17 +746,18 @@ int fed_round_small_launch(int kind, int din, int hid, int dout, const RoundPara
 }
 
 template <class Net>
-static int fits_round(int C, int M) {
+static int fits_round(int C, int M, bool server_opt) {
     const int CM = C * M, G = 8;   // the launcher may use up to the portable cluster size
-    const SmemLayout L = make_layout<Net>(M, C, (CM + G - 1) / G);
+    const SmemLayout L = make_layout<Net>(M, C, (CM + G - 1) / G, server_opt);
     return L.total * (int)sizeof(float) <= 227 * 1024;
 }
 
-// 1 when the fused kernel can run this federation: instantiated shape, t_cur < kTmax, shared-memory layout within 227 KB
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur) {
+// 1 when the fused kernel can run this federation: instantiated shape, t_cur < kTmax, shared-memory layout (with the server
+// optimizer state when server_opt) within 227 KB
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt) {
     if (t_cur >= kTmax) return 0;
 #define FDB_CASE(K, I, H, O) \
-    if (kind == K && din == I && (K == 0 || hid == H) && dout == O) return fits_round<Mlp<K, I, H, O>>(C, M);
+    if (kind == K && din == I && (K == 0 || hid == H) && dout == O) return fits_round<Mlp<K, I, H, O>>(C, M, server_opt);
     FDB_MLP_SHAPES(FDB_CASE)
 #undef FDB_CASE
     return 0;

@@ -27,6 +27,13 @@ struct RoundParams {
     float* opt_v;
     float* opt_vmax;
     int* opt_step;       // [C, M]
+    // server optimizer on the cluster models (FedOpt per slot, sopt_kind 0 = plain FedAvg): after the weighted average
+    // avg_m of a slot with total weight > 0, θ_m takes one step on g = θ_m − avg_m (common.cuh server_opt_update)
+    int sopt_kind;       // 0 none, 1 sgd(+momentum), 2 adam, 3 adagrad, 4 yogi
+    float sopt_lr, sopt_momentum, sopt_eps;
+    float* sopt_s0;      // [M, P] momentum / Adagrad sum / first moment, or nullptr (sgd without momentum)
+    float* sopt_s1;      // [M, P] second moment (adam / yogi) or nullptr
+    int* sopt_step;      // [M] steps applied per slot (Adam bias correction), advanced by every round the slot aggregates
     float* client_out;   // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs
@@ -69,7 +76,7 @@ struct SmallLaunchInfo {
 int fed_round_small_launch(int kind, int din, int hid, int dout, const RoundParams& p, int cluster, cudaStream_t stream,
                            SmallLaunchInfo* info);
 int fed_round_small_supported(int kind, int din, int hid, int dout);
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur);
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt);
 int mlp_eval_matrix_launch(int kind, int din, int hid, int dout, const float* theta, int theta_stride, int M, const float* X,
                            const int* Y, const int* nsamp, int C, int S, float* correct, float* loss, float* sqerr,
                            cudaStream_t stream);

@@ -8,7 +8,7 @@ namespace fdb {
 // aggregate.cu
 int cluster_aggregate_launch(float* theta, int theta_stride, const float* cp, const float* n, int C, int M, int P, float* tot_out,
                              int opt_kind, float lr, float momentum, float b1, float b2, float eps, int step, float* s0, float* s1,
-                             cudaStream_t stream);
+                             const int* steps, const unsigned char* mask, cudaStream_t stream);
 int weighted_average_launch(const float* rows, const float* w, int n, long long P, float* out, cudaStream_t stream);
 int merge_axpby_launch(float* base_row, const float* second_row, float w1, float w2, long long P, cudaStream_t stream);
 int sq_diff_sum_launch(const float* a, const float* b, long long P, double* out, cudaStream_t stream);

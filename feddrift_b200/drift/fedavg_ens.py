@@ -33,6 +33,7 @@ from ..core.message import DeviceRef, Message
 from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
+from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
 from .evaluator import Evaluator
@@ -400,6 +401,9 @@ class _BaseAggregator:
             for i, m in enumerate(models):
                 self.bank.load_state_dict(i, m.state_dict())
         ARENAS[self.bank.arena_id] = self.bank
+        # per-slot server optimizer (--server_optimizer): fresh state for every aggregator, i.e. every time step
+        self.bank.server_opt = make_server_opt(args, self.bank.num_models, self.bank.P, self.device,
+                                               mutils.weight_param_mask(self.bank.spec))
         self.models = [self.bank.module(i) for i in range(self.bank.num_models)]
         M, P = self.bank.num_models, self.bank.P
         self.upload = torch.zeros(worker_num, M, P, dtype=torch.float32, device=self.device)
@@ -436,7 +440,7 @@ class _BaseAggregator:
         n = self.upload_n.clone()
         if model_mask is not None:
             n[:, ~torch.as_tensor(model_mask, dtype=torch.bool, device=n.device)] = 0.0
-        ops.cluster_aggregate_(self.bank.theta, self.upload, n)
+        ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt)
 
     def aggregate(self, round_idx):
         self._aggregate_models()

@@ -50,6 +50,10 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--resume", type=int, default=0); a("--metrics_file", type=str, default=None)
     a("--use_wandb", type=int, default=0); a("--strict_ref", type=int, default=0)
     a("--rounds_per_launch", type=int, default=0)
+    # server optimizer on every cluster model (FedOpt per slot; flag names as in `main.py fedopt`), single-GPU
+    a("--server_optimizer", type=str, default="none", choices=["none", "sgd", "adam", "adagrad", "yogi"])
+    a("--server_lr", type=float, default=1.0); a("--server_momentum", type=float, default=0.0)
+    a("--server_eps", type=float, default=1e-8, help="τ of adam / adagrad / yogi")
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)
     a("--pack_workers", type=int, default=0); a("--zero_copy", type=int, default=0)
     a("--round_timeout_s", type=float, default=0.0, help="> 0: close a round without workers whose upload did not arrive in time")

@@ -48,7 +48,13 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
 
 
 # ----------------------------------------------------------------------------- K1
-def cluster_aggregate_(theta, client_params, n):
+def cluster_aggregate_(theta, client_params, n, server_opt=None):
+    """K1: θ_m ← weighted mean of ``client_params[:, m]`` for every slot with total weight > 0; returns the totals [M].
+    ``server_opt`` (``server_opt.SlotServerOpt``) then steps each such slot on θ_m − avg_m with its own state."""
+    if server_opt is not None:
+        if native(theta, client_params):
+            return server_opt.aggregate_native_(theta, client_params, n)
+        return server_opt.aggregate_reference_(theta, client_params, n)
     if native(theta, client_params):
         return _ext.load().cluster_aggregate(theta, client_params.contiguous(), n.float().contiguous())
     return ref.cluster_aggregate_(theta, client_params, n)

@@ -192,6 +192,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     ``ens_mode`` 0|1 (weighted hard vote)|2 (weighted soft vote) with ``ens_w [C,M]`` for the TEST metric.
     ``participation [rows, C]`` bool/uint8: in round ``rnd`` only the clients of row ``rnd % rows`` train and enter the
     cluster averages (a cluster with no participant keeps its model); evaluation and re-clustering still cover every client.
+    ``server_opt`` 'sgd'|'adam'|'adagrad'|'yogi' (absent or 'none': plain FedAvg) with ``server_lr`` (1.0),
+    ``server_momentum`` (0.0), ``server_eps`` (1e-8), state ``server_s0`` / ``server_s1`` [M,P] and ``server_step`` [M] int:
+    every slot whose total weight is > 0 becomes avg_m, then takes one ``server_opt_slots_`` step on θ_m − avg_m; the other
+    slots keep θ, state and counter (see ``server_opt.SlotServerOpt`` for which state rows each optimizer uses).
     Mutates theta / opt state / W (if recluster) in place; returns ``metrics [rounds, C, 4]`` =
     (train_correct, train_loss_sum, test_correct, test_loss_sum) and ``counts [C, 2]`` = (n_train, n_test).
     """
@@ -211,6 +215,9 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     part = st.get("participation")
     if part is not None:
         part = torch.as_tensor(part).to("cpu", torch.bool)
+    sopt = st.get("server_opt")
+    if sopt == "none":
+        sopt = None
     for r in range(rounds):
         rnd = round0 + r
         prow = part[rnd % part.shape[0]] if part is not None else None
@@ -249,6 +256,7 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                         p.add_(g, alpha=-cur_lr)
                 locals_[(c, m)] = (p, n_cm)
                 acc_w[m] += n_cm
+        avg = theta.clone() if sopt is not None else theta
         for m in range(M):
             if acc_w[m] <= 0:
                 continue
@@ -258,7 +266,11 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                 if (c, m) in locals_:
                     p, n_cm = locals_[(c, m)]
                     out += p * (np.float32(n_cm) / tot)
-            theta[m] = out
+            avg[m] = out
+        if sopt is not None:
+            server_opt_slots_(theta, avg, acc_w > 0, sopt, st.get("server_s0"), st.get("server_s1"), st["server_step"],
+                              float(st.get("server_lr", 1.0)), float(st.get("server_momentum", 0.0)),
+                              float(st.get("server_eps", 1e-8)))
         if st.get("recluster_hard", False):
             corr, _ = mlp_eval_matrix(theta, Xflat[t], Y[t], nsamp[t], kind, din, hid, dout)
             accm = corr / nsamp[t].clamp(min=1).float()
@@ -389,6 +401,37 @@ def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0,
     else:
         raise ValueError(opt)
     return theta
+
+
+_SLOT_STATE_KEYS = {"sgd": ("momentum", None), "adam": ("m", "v"), "adagrad": ("sum", None), "yogi": ("m", "v")}
+
+
+def server_opt_slots_(theta, avg, active, opt: str, s0, s1, steps, lr: float, momentum: float = 0.0, eps: float = 1e-8,
+                      mask=None) -> None:
+    """Per-slot FedOpt step, in place: for every slot m with ``active[m]``, θ_m takes one ``server_opt_step_`` on
+    θ_m − avg_m with the slot's own state rows ``s0[m]`` / ``s1[m]`` (None where ``opt`` has no such state) and its own step
+    count ``steps[m]`` (Adam's bias correction uses steps[m] + 1), then ``steps[m]`` advances.  Entries with ``mask`` False
+    take avg_m and keep their state.  Inactive slots are left untouched."""
+    k0, k1 = _SLOT_STATE_KEYS[opt]
+    sel = torch.ones(theta.shape[1], dtype=torch.bool, device=theta.device) if mask is None else mask.to(theta.device, torch.bool)
+    for m in range(theta.shape[0]):
+        if not bool(active[m]):
+            continue
+        th = theta[m, sel]
+        state = {"step": int(steps[m])}
+        if s0 is not None:
+            state[k0] = s0[m, sel]
+        if s1 is not None:
+            state[k1] = s1[m, sel]
+        server_opt_step_(th, avg[m, sel], state, opt, lr, momentum=momentum, eps=eps)
+        theta[m, sel] = th
+        if s0 is not None:
+            s0[m, sel] = state[k0]
+        if s1 is not None:
+            s1[m, sel] = state[k1]
+        if mask is not None:
+            theta[m, ~sel] = avg[m, ~sel]
+        steps[m] += 1
 
 
 def ada_stats(theta: torch.Tensor, prev_muh: torch.Tensor) -> float:

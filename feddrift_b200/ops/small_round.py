@@ -19,13 +19,14 @@ def supported(kind: str, din: int, hid: int, dout: int) -> bool:
     return ext is not None and bool(ext.fed_round_small_supported(KIND_ID[kind], din, hid, dout))
 
 
-def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int) -> bool:
+def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, server_opt: bool = False) -> bool:
     """True when the fused kernel can run this federation at time step ``t_cur`` (instantiated MLP shape, ``t_cur`` below
-    the kernel's plan-table limit, shared-memory layout within 227 KB); otherwise route to the generic executor."""
+    the kernel's plan-table limit, shared-memory layout — plus the ``[2, M, P]`` server optimizer state when
+    ``server_opt`` — within 227 KB); otherwise route to the generic executor."""
     ext = _ext.load()
     if ext is None:
         return True   # CPU reference has no such limits
-    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur)))
+    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt)))
 
 
 def spin_timeout_ms(st: Dict) -> int:
@@ -121,6 +122,14 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
             int(mg["rank"]) if mg else 0, int(mg["flag_base"]) if mg else 0, int(st.get("cluster", 0) or cache["cluster"]),
             spin_timeout_ms(st), int(st.get("warps_per_pair", 0) or cache["wpp"])]
     fcfg = [float(lr) if lr_dev is None else 0.0, float(st["wd"]), 0.9, 0.999, 1e-8]
+    sopt = st.get("server_opt")
+    sopt = None if sopt == "none" else sopt
+    if sopt is not None:   # per-slot server optimizer (reference.fed_round_small documents the keys)
+        from .server_opt import _KIND
+        if sopt not in _KIND:
+            raise ValueError(f"fed_round_small: unknown server optimizer {sopt!r}")
+        icfg.append(_KIND[sopt])
+        fcfg += [float(st.get("server_lr", 1.0)), float(st.get("server_momentum", 0.0)), float(st.get("server_eps", 1e-8))]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out
@@ -133,7 +142,8 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         ens_w, st.get("client_out"), lr_dev, metrics_out, st.get("timers"), fcfg, icfg,
         list(mg["inbox_ptrs"]) if mg else [], mg.get("error_flag") if mg else None,
         st.get("counters"), peer_metrics, [int(v) for v in st["host_io"]] if st.get("host_io") else [],
-        cache["participation"])
+        cache["participation"], st.get("server_s0") if sopt else None, st.get("server_s1") if sopt else None,
+        st.get("server_step") if sopt else None)
     if mg:
         mg["flag_base"] = int(mg["flag_base"]) + rounds
     if st.get("counters") is not None:

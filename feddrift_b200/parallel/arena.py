@@ -64,6 +64,9 @@ class ModelBank:
         for m in range(num_models):
             self.theta[m].copy_(self.init_row)
         self._modules: Dict[int, nn.Module] = {}
+        # per-slot server optimizer state (ops.server_opt.SlotServerOpt) or None: a slot that is re-initialised or
+        # overwritten starts its optimizer afresh, so reinit / copy reset the destination slot's state here
+        self.server_opt = None
         self.float_mask = torch.zeros(self.P, dtype=torch.bool)
         for _, _, dt, off, n in self.spec:
             self.float_mask[off:off + n] = bool(dt.is_floating_point)
@@ -93,9 +96,13 @@ class ModelBank:
     def copy(self, dst: int, src: int) -> None:
         if dst != src:
             self.theta[dst].copy_(self.theta[src])
+            if self.server_opt is not None:
+                self.server_opt.reset(dst)
 
     def reinit(self, m: int) -> None:
         self.theta[m].copy_(self.init_row)
+        if self.server_opt is not None:
+            self.server_opt.reset(m)
 
     def reset_parameters_random(self, m: int, generator: Optional[torch.Generator] = None) -> None:
         """Fresh (NOT reseeded) init — the IFCA 'hard' path at t=0 calls ``reset_parameters`` directly

@@ -35,6 +35,7 @@ from ..data.drift import DriftData, generate_drift_data
 from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
+from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
 from . import checkpoint as ckpt
@@ -47,6 +48,7 @@ DEFAULTS = dict(
     concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0", ensemble_window=4, concept_num=4,
     change_points="A", time_stretch=1, reset_models=0, noise_prob=0.0, dummy_arg=0, sample_num=100, ci=0,
     is_mobile=0, gpu_num_per_server=1, data_dir=None, checkpoint_dir=None, rounds_per_launch=0,
+    server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
 )
 
 
@@ -87,6 +89,7 @@ class DriftSim:
         mkw = {"small_input": True} if (args.model in ("resnet", "resnet18") and data.X.shape[-1] <= 64) else {}
         template = create_model(args.model, data.class_num, data.feature_num, **mkw)
         self.bank = ModelBank(template, self.M, self.device)
+        self.bank.server_opt = make_server_opt(args, self.M, self.bank.P, self.device, mutils.weight_param_mask(self.bank.spec))
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -148,6 +151,8 @@ class DriftSim:
             for m in range(self.M):
                 self.bank.reinit(m)
         self.clients.reset_optimizer()
+        if self.bank.server_opt is not None:
+            self.bank.server_opt.reset()
         self.algo.begin_step(t)
         self._small = None
         self._plan = None
@@ -196,6 +201,10 @@ class DriftSim:
                 self._small["wd"] = 0.0
             if self._participation_dev is not None:
                 self._small["participation"] = self._participation_dev
+            so = self.bank.server_opt
+            if so is not None:   # the bank's own state tensors: the kernel steps them in place
+                self._small.update(server_opt=so.opt, server_lr=so.lr, server_momentum=so.momentum, server_eps=so.eps,
+                                   server_s0=so.s0, server_s1=so.s1, server_step=so.step)
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)
@@ -209,6 +218,9 @@ class DriftSim:
     def run_rounds(self, rounds: int) -> Dict:
         """Run ``rounds`` FL rounds of the current time step; returns the last round's aggregate metrics."""
         t0 = time.perf_counter()
+        if self.bank.server_opt is not None and (self.multi is not None or getattr(self, "shard_clients", False)):
+            raise ValueError("a server optimizer (--server_optimizer) is single-GPU only: it cannot be combined with "
+                             "multi-GPU client sharding")
         done, last = 0, {}
         while done < rounds:
             block = self.algo.block_size(self.round_in_step, rounds - done)
@@ -243,7 +255,8 @@ class DriftSim:
             return True
         from ..ops import small_round
         s = self.spec
-        return small_round.fits(s["kind"], s["in"], s["hidden"], s["out"], self.C, self.M, self.t)
+        return small_round.fits(s["kind"], s["in"], s["hidden"], s["out"], self.C, self.M, self.t,
+                                server_opt=self.bank.server_opt is not None)
 
     def _check_peer_error(self) -> None:
         if self.multi is not None and self.multi["error_np"][0] != 0:
@@ -313,7 +326,9 @@ class DriftSim:
         # must not advance the experiment (models, optimizer state, RNG round counter are restored afterwards; only the
         # cross-GPU epoch stays advanced because the peers have seen it)
         cl = self.clients
-        snap = [(x, x.clone()) for x in (self.bank.theta, cl.m, cl.v, cl.vmax, cl.step, st.get("W")) if isinstance(x, torch.Tensor)]
+        so = self.bank.server_opt
+        snap = [(x, x.clone()) for x in (self.bank.theta, cl.m, cl.v, cl.vmax, cl.step, st.get("W"), *(so.tensors() if so else ()))
+                if isinstance(x, torch.Tensor)]
         cnt = st.get("counters")
         cnt0 = cnt[0:1].clone() if isinstance(cnt, torch.Tensor) else None
         r0, g0, l0 = self.round_in_step, self.global_round, small_round.LAUNCH_COUNT["fed_round_small"]

@@ -9,7 +9,8 @@ architecture and for algorithms that must look at raw client updates before aggr
   nets → ``sim/stacked.py`` (all pairs in one channel-stacked network on the grouped implicit-GEMM kernels); everything else
   per pair: bank-bound ``nn.Module`` forward/backward (TcLinear → wgmma GEMM, TcConv2d → implicit-GEMM convolution),
   gradients land in a flat scratch row, ``ops.adam_amsgrad_rows_`` / ``ops.sgd_rows_`` update the client row;
-* aggregation: ``ops.cluster_aggregate_`` over the ``[C, M, P]`` client arena (K1);
+* aggregation: ``ops.cluster_aggregate_`` over the ``[C, M, P]`` client arena (K1), with the bank's per-slot server optimizer
+  step in its epilogue when one is configured;
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -132,7 +133,7 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
             if world > 1:
                 _peer_aggregate(sim, world, rank)
             else:
-                ops.cluster_aggregate_(bank.theta, cl.params, cl.n)
+                ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt)
         if plan.get("recluster_hard"):
             acc = sim.evaluator.acc_matrix(list(range(M)), t)
             best = np.argmax(acc, axis=0)
