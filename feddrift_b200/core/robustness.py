@@ -7,7 +7,7 @@ state_dict API below is the drop-in compatible surface.
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
@@ -56,3 +56,30 @@ class RobustAggregator:
         """Rows ``[n, P]`` of client params -> clipped in place around ``global_row``."""
         from ..ops import robust_clip_
         return robust_clip_(local_rows, global_row, self.norm_bound, weight_mask)
+
+    def defend_slots_(self, upload: torch.Tensor, theta: torch.Tensor, n: torch.Tensor, weight_mask=None, seed: int = 0,
+                      rnd: int = 0) -> torch.Tensor:
+        """Apply the defense to a ``[C, M, P]`` upload arena in place before the cluster aggregation: every upload with
+        ``n[c, m] > 0`` is clipped to distance ``norm_bound`` of its slot's model ``theta[m]`` (the model it trained from)
+        and, for ``weak_dp``, gets ``stddev``-scaled ``gauss_hash`` noise of round ``rnd`` (``ops.reference.defense_seed``).
+        Entries with ``weight_mask`` False (BatchNorm statistics) pass through.  Returns the update norms ``[C, M]``."""
+        from ..ops import reference as ref, robust_clip_slots_
+        std = self.stddev if self.defense_type == "weak_dp" else 0.0
+        return robust_clip_slots_(upload, theta, n, self.norm_bound, weight_mask, std, ref.defense_seed(seed, rnd))
+
+
+def make_defense(args) -> Optional[RobustAggregator]:
+    """The robust-aggregation defense of the continual engines from ``args.defense_type`` (``none`` |
+    ``norm_diff_clipping`` | ``weak_dp``), ``args.norm_bound`` (5.0) and ``args.stddev`` (0.025, weak_dp only); None for
+    ``none``.  Raises ``ValueError`` for an unknown defense, a bound that is not finite or ≤ 0, or a negative stddev.
+
+    ``weak_dp`` is the reference's backdoor defense (clipping plus Gaussian noise on each upload): it carries no (ε, δ)
+    differential-privacy guarantee."""
+    from ..ops.reference import defense_params
+    name = str(getattr(args, "defense_type", "none") or "none")
+    bound, _ = defense_params(name, getattr(args, "norm_bound", 5.0), getattr(args, "stddev", 0.025))
+    if name == "none":
+        return None
+    ra = RobustAggregator(args)
+    ra.defense_type, ra.norm_bound, ra.stddev = name, bound, float(getattr(args, "stddev", 0.025))
+    return ra

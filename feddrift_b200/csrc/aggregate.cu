@@ -207,35 +207,33 @@ int gossip_mix_launch(const float* X, const float* Wm, int n, long long P, float
 }
 
 // ------------------------------------------------------------------------------------------------ K10
-// rows[i] <- g + (rows[i]-g) / max(1, ||mask·(rows[i]-g)|| / bound); one CTA-group per row, two passes (norm, apply);
-// the second pass re-reads the row from L2 (a 46.8 MB ResNet-18 row fits the 126 MB L2).
-__global__ void __launch_bounds__(256) row_diff_norm_kernel(const float* __restrict__ rows, const float* __restrict__ g,
-                                                            const unsigned char* __restrict__ mask, long long P, float* __restrict__ nrm2) {
+// rows[r] <- g_r + (rows[r]-g_r) / max(1, ||mask·(rows[r]-g_r)|| / bound); one CTA-group per row, two passes (norm, apply);
+// the second pass re-reads the row from L2 (a 46.8 MB ResNet-18 row fits the 126 MB L2).  Row r's anchor is
+// g_r = g + (r % M)·g_stride (the slot's model for a [C, M, P] upload arena; M = 1, g_stride = 0: one shared anchor), and
+// rows whose weight n[r] is 0 are left alone (n == nullptr: every row is clipped).
+__global__ void __launch_bounds__(256) row_diff_norm_kernel(const float* __restrict__ rows, const float* __restrict__ g, long long g_stride,
+                                                            int M, const float* __restrict__ n, const unsigned char* __restrict__ mask,
+                                                            long long P, float* __restrict__ nrm2) {
     __shared__ float red[32];
     const int r = blockIdx.y;
+    if (n && n[r] == 0.f) return;
+    const float* gr = g + (size_t)(r % M) * g_stride;
     float acc = 0.f;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < P; i += (long long)gridDim.x * blockDim.x) {
         if (mask && !mask[i]) continue;
-        const float d = rows[(size_t)r * P + i] - g[i];
+        const float d = rows[(size_t)r * P + i] - gr[i];
         acc = fmaf(d, d, acc);
     }
     acc = block_sum(acc, red);
     if (threadIdx.x == 0) atomicAdd(nrm2 + r, acc);
 }
-// counter-based N(0,1): Box–Muller on two lowbias32 hashes of (seed, row, element) — same function in ops/reference.py
-FDB_DEVICE float gauss_hash(uint32_t seed, uint32_t r, unsigned long long i) {
-    const uint32_t base = mix32(seed ^ mix32(r * 0x9E3779B9u + 0x7F4A7C15u)) ^ (uint32_t)(i >> 32) * 0x85EBCA6Bu;
-    const uint32_t h1 = mix32(base ^ ((uint32_t)i * 2u + 1u));
-    const uint32_t h2 = mix32(base ^ ((uint32_t)i * 2u + 2u) ^ 0x68E31DA4u);
-    const float u1 = ((float)(h1 >> 8) + 1.0f) * (1.0f / 16777216.0f);   // (0, 1]
-    const float u2 = (float)(h2 >> 8) * (1.0f / 16777216.0f);            // [0, 1)
-    return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
-}
-__global__ void __launch_bounds__(256) row_clip_apply_kernel(float* __restrict__ rows, const float* __restrict__ g,
-                                                             const unsigned char* __restrict__ mask, long long P,
-                                                             const float* __restrict__ nrm2, float bound, float* __restrict__ nrm_out,
-                                                             float stddev, uint32_t seed) {
+__global__ void __launch_bounds__(256) row_clip_apply_kernel(float* __restrict__ rows, const float* __restrict__ g_base, long long g_stride,
+                                                             int M, const float* __restrict__ n, const unsigned char* __restrict__ mask,
+                                                             long long P, const float* __restrict__ nrm2, float bound,
+                                                             float* __restrict__ nrm_out, float stddev, uint32_t seed) {
     const int r = blockIdx.y;
+    if (n && n[r] == 0.f) return;
+    const float* g = g_base + (size_t)(r % M) * g_stride;
     const float nrm = sqrtf(nrm2[r]);
     if (blockIdx.x == 0 && threadIdx.x == 0 && nrm_out) nrm_out[r] = nrm;
     const float scale = 1.f / fmaxf(1.f, nrm / bound);
@@ -248,12 +246,12 @@ __global__ void __launch_bounds__(256) row_clip_apply_kernel(float* __restrict__
         rows[(size_t)r * P + i] = v;
     }
 }
-int robust_clip_launch(float* rows, const float* g, const unsigned char* mask, int R, long long P, float bound, float* scratch_nrm2,
-                       float* nrm_out, float stddev, unsigned seed, cudaStream_t stream) {
+int robust_clip_launch(float* rows, const float* g, long long g_stride, int M, const float* n, const unsigned char* mask, int R,
+                       long long P, float bound, float* scratch_nrm2, float* nrm_out, float stddev, unsigned seed, cudaStream_t stream) {
     cudaMemsetAsync(scratch_nrm2, 0, R * sizeof(float), stream);
     dim3 grid(max(1, persistent_grid(P, 256) / max(1, min(R, 16))), R);
-    row_diff_norm_kernel<<<grid, 256, 0, stream>>>(rows, g, mask, P, scratch_nrm2);
-    row_clip_apply_kernel<<<grid, 256, 0, stream>>>(rows, g, mask, P, scratch_nrm2, bound, nrm_out, stddev, seed);
+    row_diff_norm_kernel<<<grid, 256, 0, stream>>>(rows, g, g_stride, M, n, mask, P, scratch_nrm2);
+    row_clip_apply_kernel<<<grid, 256, 0, stream>>>(rows, g, g_stride, M, n, mask, P, scratch_nrm2, bound, nrm_out, stddev, seed);
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 

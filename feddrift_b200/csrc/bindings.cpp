@@ -49,7 +49,7 @@ std::vector<int64_t> fed_round_small(
     p.lr_ptr = opt_ptr<float>(lr_dev);
     p.metrics = metrics.data_ptr<float>();
     p.timers = (timers.has_value() && timers->defined()) ? reinterpret_cast<long long*>(timers->data_ptr<int64_t>()) : nullptr;
-    // fcfg: lr, wd, beta1, beta2, eps [, server_lr, server_momentum, server_eps]
+    // fcfg: lr, wd, beta1, beta2, eps [, server_lr, server_momentum, server_eps [, defense norm bound, defense stddev]]
     p.lr = (float)fcfg[0]; p.wd = (float)fcfg[1]; p.beta1 = (float)fcfg[2]; p.beta2 = (float)fcfg[3]; p.eps = (float)fcfg[4];
     // icfg: T1, C, S, M, Lmax, batch, epochs, t_cur, rounds, round0, seed, use_adam, sample_mode, n_mode, recluster, ens_mode,
     //       skip_aggregate, world, rank, flag_base, cluster, spin_timeout_ms, warps_per_pair [, server optimizer kind]
@@ -117,6 +117,13 @@ std::vector<int64_t> fed_round_small(
                     ss.dim() == 1 && ss.size(0) == M,
                     "fed_round_small: server_step must be a contiguous int32 [M] tensor on the device of X");
         p.sopt_step = ss.data_ptr<int>();
+    }
+    if (fcfg.size() >= 10) {   // robust aggregation: fcfg[8] = norm bound (0 = off), fcfg[9] = weak-DP noise stddev
+        TORCH_CHECK(std::isfinite(fcfg[8]) && fcfg[8] >= 0.0, "fed_round_small: the defense norm bound must be finite and > 0 (0 = off)");
+        TORCH_CHECK(std::isfinite(fcfg[9]) && fcfg[9] >= 0.0, "fed_round_small: the defense stddev must be finite and >= 0");
+        TORCH_CHECK(fcfg[8] > 0.0 || fcfg[9] == 0.0, "fed_round_small: weak-DP noise needs a norm bound > 0");
+        p.def_bound = (float)fcfg[8]; p.def_stddev = (float)fcfg[9];
+        TORCH_CHECK(fcfg[8] == 0.0 || p.def_bound > 0.f, "fed_round_small: the defense norm bound underflows float32");
     }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
@@ -249,8 +256,44 @@ Tensor robust_clip(Tensor rows, Tensor g, double bound, c10::optional<Tensor> ma
     const int R = (int)rows.size(0);
     auto scratch = torch::zeros({R}, rows.options());
     auto nrm = torch::zeros({R}, rows.options());
-    CHECK_OK(fdb::robust_clip_launch(rows.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<unsigned char>(mask), R, rows.size(1), (float)bound,
-                                     scratch.data_ptr<float>(), nrm.data_ptr<float>(), (float)stddev, (unsigned)seed, cur_stream()), "robust_clip");
+    CHECK_OK(fdb::robust_clip_launch(rows.data_ptr<float>(), g.data_ptr<float>(), 0, 1, nullptr, opt_ptr<unsigned char>(mask), R, rows.size(1),
+                                     (float)bound, scratch.data_ptr<float>(), nrm.data_ptr<float>(), (float)stddev, (unsigned)seed, cur_stream()),
+             "robust_clip");
+    return nrm;
+}
+
+// K10 over an upload arena rows [C, M, P] (contiguous): row (c, m) is clipped around its slot's model theta[m, :P] (theta
+// [M, stride >= P], unit column stride, e.g. a padded ModelBank) and, when stddev > 0, gets stddev·gauss_hash(seed, c·M + m, e)
+// on every masked entry e.  Rows whose weight n[c, m] is 0 are left untouched.  Returns the clip norms [C·M] (0 for skipped rows).
+Tensor robust_clip_slots(Tensor rows, Tensor theta, c10::optional<Tensor> n, double bound, c10::optional<Tensor> mask, double stddev,
+                         int64_t seed) {
+    CHECK_CUDA_F32(rows); CHECK_CUDA_F32(theta);
+    TORCH_CHECK(rows.is_contiguous() && rows.dim() == 3, "robust_clip_slots: rows must be a contiguous [C, M, P] tensor");
+    const int64_t M = rows.size(1), P = rows.size(2), R = rows.size(0) * M;
+    TORCH_CHECK(M >= 1 && R <= 65535, "robust_clip_slots: need M >= 1 and at most 65535 rows (one grid row each)");
+    TORCH_CHECK(theta.device() == rows.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "robust_clip_slots: theta must be [M, >= P] with unit column stride on the device of rows");
+    TORCH_CHECK(std::isfinite(bound) && bound > 0.0, "robust_clip_slots: bound must be finite and > 0");
+    TORCH_CHECK(std::isfinite(stddev) && stddev >= 0.0, "robust_clip_slots: stddev must be finite and >= 0");
+    const float* np_ = nullptr;
+    if (n.has_value() && n->defined()) {
+        TORCH_CHECK(n->is_cuda() && n->device() == rows.device() && n->scalar_type() == torch::kFloat32 && n->is_contiguous() &&
+                    n->numel() == R, "robust_clip_slots: n must be a contiguous float32 [C, M] tensor on the device of rows");
+        np_ = n->data_ptr<float>();
+    }
+    const unsigned char* mp = nullptr;
+    if (mask.has_value() && mask->defined()) {
+        TORCH_CHECK(mask->is_cuda() && mask->device() == rows.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                    mask->numel() >= P, "robust_clip_slots: mask must be a contiguous uint8 [>= P] tensor on the device of rows");
+        mp = mask->data_ptr<unsigned char>();
+    }
+    c10::cuda::CUDAGuard guard(rows.device());
+    auto scratch = torch::zeros({R}, rows.options());
+    auto nrm = torch::zeros({R}, rows.options());
+    if (R == 0 || P == 0) return nrm;
+    CHECK_OK(fdb::robust_clip_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)M, np_, mp, (int)R, P,
+                                     (float)bound, scratch.data_ptr<float>(), nrm.data_ptr<float>(), (float)stddev, (unsigned)seed,
+                                     cur_stream()), "robust_clip_slots");
     return nrm;
 }
 
@@ -851,6 +894,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("mean_sq_diff", &mean_sq_diff);
     m.def("gossip_mix", &gossip_mix);
     m.def("robust_clip", &robust_clip);
+    m.def("robust_clip_slots", &robust_clip_slots);
     m.def("eval_logits", &eval_logits);
     m.def("aue_sqerr", &aue_sqerr);
     m.def("ensemble_vote", &ensemble_vote);

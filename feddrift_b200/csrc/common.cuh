@@ -21,6 +21,18 @@ FDB_HOST_DEVICE uint32_t batch_hash(uint32_t seed, uint32_t rnd, uint32_t client
     return h;
 }
 FDB_DEVICE uint32_t hash_choice(uint32_t h, uint32_t n) { return __umulhi(h, n); }
+// counter-based N(0,1): Box–Muller on two lowbias32 hashes of (seed, row, element) — same function in ops/reference.py
+FDB_DEVICE float gauss_hash(uint32_t seed, uint32_t r, unsigned long long i) {
+    const uint32_t base = mix32(seed ^ mix32(r * 0x9E3779B9u + 0x7F4A7C15u)) ^ (uint32_t)(i >> 32) * 0x85EBCA6Bu;
+    const uint32_t h1 = mix32(base ^ ((uint32_t)i * 2u + 1u));
+    const uint32_t h2 = mix32(base ^ ((uint32_t)i * 2u + 2u) ^ 0x68E31DA4u);
+    const float u1 = ((float)(h1 >> 8) + 1.0f) * (1.0f / 16777216.0f);   // (0, 1]
+    const float u2 = (float)(h2 >> 8) * (1.0f / 16777216.0f);            // [0, 1)
+    return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
+}
+// gauss_hash seed of the weak-DP noise of round `rnd` of a time step whose engine seed is `seed` (ops/reference.py
+// defense_seed); the noise of (client c, slot m) is gauss_hash(defense_seed(seed, rnd), c·M + m, element)
+FDB_HOST_DEVICE uint32_t defense_seed(uint32_t seed, uint32_t rnd) { return mix32(seed ^ mix32(rnd * 0xC2B2AE35u + 0x2545F491u)); }
 
 // ---------------------------------------------------------------- warp reductions
 FDB_DEVICE float warp_sum(float v) {

@@ -87,7 +87,9 @@ struct BatchSel {
     const int* list; // mode 2: flat sample ids
 };
 
-template <class Net>
+// kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
+// its code and register allocation
+template <class Net, bool kDefend>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P, IN = Net::kIn, OUT = Net::kOut, HID = Net::kHid;
@@ -414,12 +416,33 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     if (lane == 0) p.opt_step[c * M + m] = ostep;
                 }
                 const float wgt = ncm_s[k] / tot_s[m];
+                float dscale = 1.f;
+                bool defend = false;
+                if constexpr (kDefend) {
+                    // robust aggregation: clip the update thl − θ_m (θ_s still holds the round-start models) to norm def_bound
+                    // and, with weak DP, add noise; s == 1 without noise publishes the local model unchanged (K10's early exit)
+                    float ss = 0.f;
+#pragma unroll
+                    for (int q = 0; q < COLS; ++q) {
+                        const int pp = lane + 32 * q;
+                        if (pp < P) { const float d = thl[pp] - theta_s[m * P + pp]; ss = fmaf(d, d, ss); }
+                    }
+                    dscale = 1.f / fmaxf(1.f, sqrtf(warp_sum(ss)) / p.def_bound);
+                    defend = dscale != 1.f || p.def_stddev != 0.f;
+                }
 #pragma unroll
                 for (int q = 0; q < COLS; ++q) {
                     const int pp = lane + 32 * q;
                     if (pp < P) {
-                        slot_s[li * P + pp] = thl[pp] * wgt;
-                        if (p.client_out && r == p.rounds - 1) p.client_out[obase + pp] = thl[pp];
+                        float v = thl[pp];
+                        if (kDefend && defend) {
+                            const float th0 = theta_s[m * P + pp];
+                            v = th0 + (v - th0) * dscale;
+                            if (p.def_stddev != 0.f)
+                                v = fmaf(p.def_stddev, gauss_hash(defense_seed(p.seed, rnd), (uint32_t)k, (unsigned long long)pp), v);
+                        }
+                        slot_s[li * P + pp] = v * wgt;
+                        if (p.client_out && r == p.rounds - 1) p.client_out[obase + pp] = thl[pp];   // the raw local model
                     }
                 }
                 if (lane == 0) slot_model[li] = m;
@@ -716,7 +739,7 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     const SmemLayout L = make_layout<Net>(p.M, p.C, pairs_per_cta, p.sopt_kind != 0);
     const int smem = L.total * (int)sizeof(float);
     if (smem > 227 * 1024) return -2;
-    auto kern = fed_round_small_kernel<Net>;
+    auto kern = p.def_bound > 0.f ? fed_round_small_kernel<Net, true> : fed_round_small_kernel<Net, false>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return -3;
     cudaLaunchConfig_t cfg{};

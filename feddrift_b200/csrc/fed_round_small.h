@@ -34,6 +34,9 @@ struct RoundParams {
     float* sopt_s0;      // [M, P] momentum / Adagrad sum / first moment, or nullptr (sgd without momentum)
     float* sopt_s1;      // [M, P] second moment (adam / yogi) or nullptr
     int* sopt_step;      // [M] steps applied per slot (Adam bias correction), advanced by every round the slot aggregates
+    // robust aggregation (def_bound 0 = off): each pair's upload x enters its slot's average as θ_m + s·(x − θ_m),
+    // s = 1 / max(1, ‖x − θ_m‖ / def_bound), plus def_stddev·gauss_hash(defense_seed(seed, round), c·M + m, e) (weak DP)
+    float def_bound, def_stddev;
     float* client_out;   // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs

@@ -16,8 +16,9 @@ int gossip_mix_launch(const float* X, const float* Wm, int n, long long P, float
 int gossip_mix_peer_launch(const long long* x_ptrs, const long long* flag_ptrs, const float* w, int P, int world, int rank,
                            unsigned* grid_sync, unsigned grid_base, unsigned epoch, int grid, long long timeout_ms, int* error_flag,
                            cudaStream_t stream);
-int robust_clip_launch(float* rows, const float* g, const unsigned char* mask, int R, long long P, float bound, float* scratch_nrm2,
-                       float* nrm_out, float stddev, unsigned seed, cudaStream_t stream);
+// K10: row r of rows [R, P] is clipped around g + (r % M)·g_stride; rows with n[r] == 0 are skipped (n may be nullptr)
+int robust_clip_launch(float* rows, const float* g, long long g_stride, int M, const float* n, const unsigned char* mask, int R,
+                       long long P, float bound, float* scratch_nrm2, float* nrm_out, float stddev, unsigned seed, cudaStream_t stream);
 // aggregate_peer.cu : multi-GPU reduce-scatter + apply + all-gather over NVLink peer memory (cooperative launch)
 int fedavg_reduce_apply_peer_launch(const float* cp, const int* cidx, const float* n, int C, int M, int P, int theta_stride, int world, int rank,
                                     const long long* part_ptrs, const long long* theta_ptrs, const long long* tot_ptrs,

@@ -33,6 +33,7 @@ from ..core.message import DeviceRef, Message
 from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
+from ..core.robustness import make_defense
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
@@ -385,6 +386,8 @@ class FedAvgEnsTrainerClusterFL(FedAvgEnsTrainer):
 class _BaseAggregator:
     """Bookkeeping + K1 aggregation shared by every ``FedAvgEnsAggregator*``."""
 
+    defend_uploads = True   # apply ``--defense_type`` in ``_aggregate_models`` (single-model FedAvg defends in its own hook)
+
     def __init__(self, train_globals, test_globals, all_train_data_nums, train_data_local_dicts, test_data_local_dicts,
                  train_data_local_num_dicts, all_data, worker_num, device, models, class_num, args):
         self.train_globals, self.test_globals = train_globals, test_globals
@@ -402,8 +405,12 @@ class _BaseAggregator:
                 self.bank.load_state_dict(i, m.state_dict())
         ARENAS[self.bank.arena_id] = self.bank
         # per-slot server optimizer (--server_optimizer): fresh state for every aggregator, i.e. every time step
-        self.bank.server_opt = make_server_opt(args, self.bank.num_models, self.bank.P, self.device,
-                                               mutils.weight_param_mask(self.bank.spec))
+        wmask = mutils.weight_param_mask(self.bank.spec)[: self.bank.P]
+        self.bank.server_opt = make_server_opt(args, self.bank.num_models, self.bank.P, self.device, wmask)
+        # robust aggregation (--defense_type) of the uploads; its noise round counts this aggregator's aggregations
+        self.defense = make_defense(args) if self.defend_uploads else None
+        self.defense_mask = None if bool(wmask.all()) else wmask.to(self.device)
+        self._defense_round = 0
         self.models = [self.bank.module(i) for i in range(self.bank.num_models)]
         M, P = self.bank.num_models, self.bank.P
         self.upload = torch.zeros(worker_num, M, P, dtype=torch.float32, device=self.device)
@@ -440,6 +447,11 @@ class _BaseAggregator:
         n = self.upload_n.clone()
         if model_mask is not None:
             n[:, ~torch.as_tensor(model_mask, dtype=torch.bool, device=n.device)] = 0.0
+        if self.defense is not None:   # row = worker index · M + m; the engine's seed of this time step
+            self._defense_round += 1
+            a = self.args
+            seed = int(getattr(a, "dummy_arg", 0)) * 7919 + 13 + 1000003 * int(getattr(a, "curr_train_iteration", 0) or 0)
+            self.defense.defend_slots_(self.upload, self.bank.theta, n, self.defense_mask, seed, self._defense_round)
         ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt)
 
     def aggregate(self, round_idx):

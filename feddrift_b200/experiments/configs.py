@@ -20,6 +20,11 @@ CONFIGS = {
                                                       concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
                                                       concept_num=4, change_points="A", sample_num=100, batch_size=500,
                                                       comm_round=40, server_optimizer="adam", server_lr=0.03, server_eps=1e-3),
+    # config 2 with the weak-DP defense: every upload is clipped to norm 5 around its cluster model and noised before averaging
+    "cfg2d_sea_fnn_100clients_weakdp_feddrift": dict(model="fnn", dataset="sea", client_num_in_total=100, client_num_per_round=100,
+                                                     concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
+                                                     concept_num=4, change_points="A", sample_num=100, batch_size=500,
+                                                     comm_round=40, defense_type="weak_dp", norm_bound=5.0, stddev=0.025),
     # config 3: MNIST 2-conv CNN, 4 concepts, 64 clients, IFCA hard-r
     "cfg3_mnist_cnn_64clients_ifca": dict(model="cnn", dataset="MNIST", client_num_in_total=64, client_num_per_round=64,
                                           concept_drift_algo="softclusterwin-1", concept_drift_algo_arg="hard-r", concept_num=4,

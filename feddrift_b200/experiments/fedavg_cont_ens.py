@@ -54,6 +54,10 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--server_optimizer", type=str, default="none", choices=["none", "sgd", "adam", "adagrad", "yogi"])
     a("--server_lr", type=float, default=1.0); a("--server_momentum", type=float, default=0.0)
     a("--server_eps", type=float, default=1e-8, help="τ of adam / adagrad / yogi")
+    # robust aggregation of every upload before its cluster average (flag names as in `main.py fedavg_robust`); weak_dp is
+    # the reference's backdoor defense (clipping + Gaussian noise) and carries no (ε, δ) privacy guarantee
+    a("--defense_type", type=str, default="none", choices=["none", "norm_diff_clipping", "weak_dp"])
+    a("--norm_bound", type=float, default=5.0); a("--stddev", type=float, default=0.025, help="weak_dp noise stddev")
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)
     a("--pack_workers", type=int, default=0); a("--zero_copy", type=int, default=0)
     a("--round_timeout_s", type=float, default=0.0, help="> 0: close a round without workers whose upload did not arrive in time")

@@ -111,6 +111,8 @@ class FedAVGTrainer:
 class FedAVGAggregator(_BaseAggregator):
     """Server side of single-model FedAvg (parity: ``FedAVGAggregator.py:13-178``)."""
 
+    defend_uploads = False   # ``fedavg_robust`` applies its defense in ``_prepare_uploads``
+
     def __init__(self, train_global, test_global, all_train_data_num, train_data_local_dict, test_data_local_dict,
                  train_data_local_num_dict, worker_num, device, model, args):
         super().__init__([train_global], [test_global], [all_train_data_num], [train_data_local_dict], [test_data_local_dict],

@@ -12,7 +12,7 @@ Kernel map (SURVEY §2.9 numbering):
   K6  gram_cosine                                 csrc/cluster_ops.cu
   K7  aue_sqerr / ensemble_vote / confusion       csrc/eval.cu
   K8  ada_stats (fused mean-square)               csrc/aggregate.cu
-  K10 robust_clip_                                csrc/aggregate.cu
+  K10 robust_clip_ / robust_clip_slots_           csrc/aggregate.cu
   K11 server_opt_step_                            csrc/aggregate.cu
   K12 gossip_mix                                  csrc/aggregate.cu
   K13 modp_matmul                                 csrc/mpc.cu
@@ -77,6 +77,18 @@ def robust_clip_(rows, global_row, bound: float, weight_mask=None, stddev: float
         mask = weight_mask.to(torch.uint8).contiguous() if weight_mask is not None else None
         return _ext.load().robust_clip(rows, global_row.contiguous(), float(bound), mask, float(stddev), int(seed) & 0xFFFFFFFF)
     return ref.robust_clip_(rows, global_row, bound, weight_mask, stddev, seed)
+
+
+def robust_clip_slots_(rows, theta, n=None, bound: float = 5.0, weight_mask=None, stddev: float = 0.0, seed: int = 0):
+    """K10 over an upload arena ``rows [C, M, P]``: every row with ``n[c, m] > 0`` is clipped around its slot's model
+    ``theta[m, :P]`` (``theta`` may be a padded bank) and, with ``stddev > 0``, gets ``gauss_hash(seed, c·M + m, ·)`` noise.
+    See ``reference.robust_clip_slots_``; returns the norms ``[C, M]``."""
+    if native(rows, theta):
+        mask = weight_mask[: rows.shape[2]].to(torch.uint8).contiguous() if weight_mask is not None else None
+        nn = n.float().contiguous() if n is not None else None
+        out = _ext.load().robust_clip_slots(rows, theta, nn, float(bound), mask, float(stddev), int(seed) & 0xFFFFFFFF)
+        return out.view(rows.shape[0], rows.shape[1])
+    return ref.robust_clip_slots_(rows, theta, n, bound, weight_mask, stddev, seed)
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, **kw):

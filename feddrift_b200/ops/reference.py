@@ -196,6 +196,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     ``server_momentum`` (0.0), ``server_eps`` (1e-8), state ``server_s0`` / ``server_s1`` [M,P] and ``server_step`` [M] int:
     every slot whose total weight is > 0 becomes avg_m, then takes one ``server_opt_slots_`` step on θ_m − avg_m; the other
     slots keep θ, state and counter (see ``server_opt.SlotServerOpt`` for which state rows each optimizer uses).
+    ``defense`` 'norm_diff_clipping'|'weak_dp' (absent or 'none': off) with ``norm_bound`` (5.0) and ``stddev`` (0.025, weak_dp
+    only): before the average, every trained pair's local model goes through ``robust_clip_slots_`` against the round-start θ
+    with seed ``defense_seed(seed, rnd)``; the weights are unchanged.  ``client_out [C, M, P]``: the raw (undefended) local
+    models of the pairs that trained in the last round are written there.
     Mutates theta / opt state / W (if recluster) in place; returns ``metrics [rounds, C, 4]`` =
     (train_correct, train_loss_sum, test_correct, test_loss_sum) and ``counts [C, 2]`` = (n_train, n_test).
     """
@@ -218,6 +222,9 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     sopt = st.get("server_opt")
     if sopt == "none":
         sopt = None
+    defense = st.get("defense") or "none"
+    def_bound, def_std = defense_params(defense, st.get("norm_bound", 5.0), st.get("stddev", 0.025))
+    client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
         prow = part[rnd % part.shape[0]] if part is not None else None
@@ -256,6 +263,17 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                         p.add_(g, alpha=-cur_lr)
                 locals_[(c, m)] = (p, n_cm)
                 acc_w[m] += n_cm
+                if client_out is not None and r == rounds - 1:
+                    client_out[c, m] = p
+        if defense != "none" and locals_:
+            up = torch.zeros(C, M, P, dtype=torch.float32)
+            for (c, m), (p, _) in locals_.items():
+                up[c, m] = p
+            trained = torch.zeros(C, M)
+            for (c, m) in locals_:
+                trained[c, m] = 1.0
+            robust_clip_slots_(up, theta, trained, def_bound, None, def_std, defense_seed(seed, rnd))
+            locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
         avg = theta.clone() if sopt is not None else theta
         for m in range(M):
             if acc_w[m] <= 0:
@@ -340,11 +358,15 @@ def _mix32_np(x):
 
 def gauss_hash(seed: int, R: int, P: int) -> torch.Tensor:
     """[R, P] standard-normal noise: Box–Muller on lowbias32 hashes of (seed, row, element) — bit-compatible inputs
-    with ``gauss_hash`` in csrc/aggregate.cu (P < 2³²)."""
-    import numpy as np
+    with ``gauss_hash`` in csrc/common.cuh (P < 2³²)."""
+    return gauss_hash_rows(seed, np.arange(R), P)
+
+
+def gauss_hash_rows(seed: int, rows, P: int) -> torch.Tensor:
+    """``gauss_hash`` noise of the listed row ids only: ``[len(rows), P]``."""
     with np.errstate(over="ignore"):
         i = np.arange(P, dtype=np.uint32)[None, :]
-        r = np.arange(R, dtype=np.uint32)[:, None]
+        r = np.asarray(rows, dtype=np.uint32).reshape(-1, 1)
         base = _mix32_np(np.uint32(seed & M32) ^ _mix32_np(r * np.uint32(0x9E3779B9) + np.uint32(0x7F4A7C15)))
         h1 = _mix32_np(base ^ (i * np.uint32(2) + np.uint32(1)))
         h2 = _mix32_np(base ^ (i * np.uint32(2) + np.uint32(2)) ^ np.uint32(0x68E31DA4))
@@ -367,6 +389,58 @@ def robust_clip_(rows: torch.Tensor, global_row: torch.Tensor, bound: float, wei
         new = torch.where(weight_mask.bool(), new, rows)
     rows.copy_(new)
     return norm.squeeze(1)
+
+
+DEFENSES = ("none", "norm_diff_clipping", "weak_dp")
+
+
+def defense_params(defense: str, norm_bound: float, stddev: float) -> Tuple[float, float]:
+    """Validated ``(norm_bound, noise stddev)`` of a robust-aggregation defense (``--defense_type`` / ``--norm_bound`` /
+    ``--stddev``); the stddev is 0 unless ``defense`` is ``weak_dp``.  Raises ``ValueError`` for an unknown defense, a
+    bound that is not finite or ≤ 0, or a negative stddev."""
+    if defense not in DEFENSES:
+        raise ValueError(f"defense_type must be one of {', '.join(DEFENSES)} (got {defense!r})")
+    bound, std = float(norm_bound), float(stddev)
+    if not math.isfinite(bound) or bound <= 0.0:
+        raise ValueError(f"norm_bound must be finite and > 0 (got {norm_bound!r})")
+    if not math.isfinite(std) or std < 0.0:
+        raise ValueError(f"stddev must be finite and >= 0 (got {stddev!r})")
+    return bound, (std if defense == "weak_dp" else 0.0)
+
+
+def defense_seed(seed: int, rnd: int) -> int:
+    """``gauss_hash`` seed of the weak-DP noise in round ``rnd`` of a time step whose engine seed is ``seed`` (the
+    ``defense_seed`` of csrc/common.cuh): a function of (seed, round) only, so resumed runs, multi-round launches and
+    CUDA-graph replays draw the same noise."""
+    return mix32((seed & M32) ^ mix32((rnd * 0xC2B2AE35 + 0x2545F491) & M32))
+
+
+def robust_clip_slots_(rows: torch.Tensor, theta: torch.Tensor, n=None, bound: float = 5.0, weight_mask=None,
+                       stddev: float = 0.0, seed: int = 0) -> torch.Tensor:
+    """K10 over an upload arena ``rows [C, M, P]``, in place: row (c, m) with ``n[c, m] > 0`` (every row when ``n`` is None)
+    becomes θ_m + s·(row − θ_m) with s = 1 / max(1, ‖mask·(row − θ_m)‖ / bound) and θ_m = ``theta[m, :P]``, plus
+    ``stddev · gauss_hash(seed, c·M + m, e)`` on every entry e.  Entries with ``weight_mask`` False pass through; a row with
+    s == 1 and no noise is left bit-identical.  Returns the norms ``[C, M]`` (0 for skipped rows)."""
+    C, M, P = rows.shape
+    th = theta[:, :P].to(rows.device)
+    sel = torch.ones(C, M, dtype=torch.bool) if n is None else (n.detach().cpu().reshape(C, M) > 0)
+    wm = None if weight_mask is None else weight_mask[:P].to(rows.device).bool()
+    norms = torch.zeros(C, M, dtype=torch.float32, device=rows.device)
+    for c, m in sel.nonzero().tolist():
+        row = rows[c, m]
+        diff = row - th[m]
+        nrm = (diff if wm is None else diff * wm).norm()
+        norms[c, m] = nrm
+        scale = 1.0 / torch.clamp(nrm / bound, min=1.0)
+        if bool(scale == 1.0) and not stddev:
+            continue
+        new = th[m] + diff * scale
+        if stddev:
+            new = new + stddev * gauss_hash_rows(seed, [c * M + m], P)[0].to(rows.device)
+        if wm is not None:
+            new = torch.where(wm, new, row)
+        row.copy_(new)
+    return norms
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

@@ -130,6 +130,12 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
             raise ValueError(f"fed_round_small: unknown server optimizer {sopt!r}")
         icfg.append(_KIND[sopt])
         fcfg += [float(st.get("server_lr", 1.0)), float(st.get("server_momentum", 0.0)), float(st.get("server_eps", 1e-8))]
+    defense = st.get("defense") or "none"
+    if defense != "none":   # robust aggregation in the publish step (reference.fed_round_small documents the keys)
+        from .reference import defense_params
+        if len(fcfg) == 5:
+            fcfg += [1.0, 0.0, 1e-8]   # server optimizer slots, unread without one
+        fcfg += list(defense_params(defense, st.get("norm_bound", 5.0), st.get("stddev", 0.025)))
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out

@@ -35,6 +35,7 @@ from ..data.drift import DriftData, generate_drift_data
 from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
+from ..core.robustness import make_defense
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -49,6 +50,7 @@ DEFAULTS = dict(
     change_points="A", time_stretch=1, reset_models=0, noise_prob=0.0, dummy_arg=0, sample_num=100, ci=0,
     is_mobile=0, gpu_num_per_server=1, data_dir=None, checkpoint_dir=None, rounds_per_launch=0,
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
+    defense_type="none", norm_bound=5.0, stddev=0.025,
 )
 
 
@@ -89,7 +91,11 @@ class DriftSim:
         mkw = {"small_input": True} if (args.model in ("resnet", "resnet18") and data.X.shape[-1] <= 64) else {}
         template = create_model(args.model, data.class_num, data.feature_num, **mkw)
         self.bank = ModelBank(template, self.M, self.device)
-        self.bank.server_opt = make_server_opt(args, self.M, self.bank.P, self.device, mutils.weight_param_mask(self.bank.spec))
+        wmask = mutils.weight_param_mask(self.bank.spec)
+        self.bank.server_opt = make_server_opt(args, self.M, self.bank.P, self.device, wmask)
+        # robust aggregation (--defense_type): uploads are clipped (+ noised) against the round-start models before averaging
+        self.defense = make_defense(args)
+        self.defense_mask = None if bool(wmask[: self.bank.P].all()) else wmask[: self.bank.P].to(self.device)
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -205,6 +211,8 @@ class DriftSim:
             if so is not None:   # the bank's own state tensors: the kernel steps them in place
                 self._small.update(server_opt=so.opt, server_lr=so.lr, server_momentum=so.momentum, server_eps=so.eps,
                                    server_s0=so.s0, server_s1=so.s1, server_step=so.step)
+            if self.defense is not None:
+                self._small.update(defense=self.defense.defense_type, norm_bound=self.defense.norm_bound, stddev=self.defense.stddev)
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)

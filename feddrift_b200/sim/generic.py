@@ -10,7 +10,8 @@ architecture and for algorithms that must look at raw client updates before aggr
   per pair: bank-bound ``nn.Module`` forward/backward (TcLinear → wgmma GEMM, TcConv2d → implicit-GEMM convolution),
   gradients land in a flat scratch row, ``ops.adam_amsgrad_rows_`` / ``ops.sgd_rows_`` update the client row;
 * aggregation: ``ops.cluster_aggregate_`` over the ``[C, M, P]`` client arena (K1), with the bank's per-slot server optimizer
-  step in its epilogue when one is configured;
+  step in its epilogue when one is configured; a robust-aggregation defense first clips (+ noises) the arena rows in place
+  (``ops.robust_clip_slots_``, K10) after the raw-update hooks have seen them;
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -130,6 +131,8 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
         if hasattr(sim.algo, "on_client_updates") and not sim.algo.split_done and rnd == sim.algo.split_round:
             sim.algo.on_client_updates(t, cl.params, cl.n)
         if not skip:
+            if sim.defense is not None:   # robust aggregation: clip (+ noise) the uploads against the round-start models
+                sim.defense.defend_slots_(cl.params, bank.theta, cl.n, sim.defense_mask, seed, rnd)
             if world > 1:
                 _peer_aggregate(sim, world, rank)
             else:
