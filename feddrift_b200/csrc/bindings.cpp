@@ -49,7 +49,8 @@ std::vector<int64_t> fed_round_small(
     p.lr_ptr = opt_ptr<float>(lr_dev);
     p.metrics = metrics.data_ptr<float>();
     p.timers = (timers.has_value() && timers->defined()) ? reinterpret_cast<long long*>(timers->data_ptr<int64_t>()) : nullptr;
-    // fcfg: lr, wd, beta1, beta2, eps [, server_lr, server_momentum, server_eps [, defense norm bound, defense stddev]]
+    // fcfg: lr, wd, beta1, beta2, eps [, server_lr, server_momentum, server_eps [, defense norm bound, defense stddev
+    //       [, fedprox mu]]]
     p.lr = (float)fcfg[0]; p.wd = (float)fcfg[1]; p.beta1 = (float)fcfg[2]; p.beta2 = (float)fcfg[3]; p.eps = (float)fcfg[4];
     // icfg: T1, C, S, M, Lmax, batch, epochs, t_cur, rounds, round0, seed, use_adam, sample_mode, n_mode, recluster, ens_mode,
     //       skip_aggregate, world, rank, flag_base, cluster, spin_timeout_ms, warps_per_pair [, server optimizer kind]
@@ -124,6 +125,11 @@ std::vector<int64_t> fed_round_small(
         TORCH_CHECK(fcfg[8] > 0.0 || fcfg[9] == 0.0, "fed_round_small: weak-DP noise needs a norm bound > 0");
         p.def_bound = (float)fcfg[8]; p.def_stddev = (float)fcfg[9];
         TORCH_CHECK(fcfg[8] == 0.0 || p.def_bound > 0.f, "fed_round_small: the defense norm bound underflows float32");
+    }
+    if (fcfg.size() >= 11) {   // FedProx: fcfg[10] = proximal coefficient mu (0 = off)
+        TORCH_CHECK(std::isfinite(fcfg[10]) && fcfg[10] >= 0.0, "fed_round_small: fedprox_mu must be finite and >= 0");
+        p.prox_mu = (float)fcfg[10];
+        TORCH_CHECK(std::isfinite(p.prox_mu), "fed_round_small: fedprox_mu overflows float32");
     }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
@@ -380,21 +386,68 @@ Tensor confusion_matrix(Tensor pred, Tensor target, int64_t classes) {
 }
 
 // ---------------------------------------------------------------------------------- optimizers
+// FedProx anchor of the row optimizers: anchor [A, >= P] (unit column stride, e.g. a padded ModelBank), anchor_rows int32 [R]
+// (optimizer row r -> anchor row), prox_mask uint8 [>= P] or none; no anchor = off
+fdb::ProxAnchor prox_anchor(const char* who, const Tensor& p, int64_t R, int64_t P, double mu, const c10::optional<Tensor>& anchor,
+                            const c10::optional<Tensor>& anchor_rows, const c10::optional<Tensor>& prox_mask) {
+    fdb::ProxAnchor px{};
+    if (!(anchor.has_value() && anchor->defined())) return px;
+    TORCH_CHECK(std::isfinite(mu) && mu >= 0.0 && std::isfinite((float)mu), who, ": fedprox mu must be finite and >= 0");
+    const Tensor& a = *anchor;
+    TORCH_CHECK(a.is_cuda() && a.device() == p.device() && a.scalar_type() == torch::kFloat32 && a.dim() == 2 && a.size(1) >= P &&
+                    a.stride(1) == 1, who, ": the prox anchor must be a float32 [A, >= P] tensor with unit column stride on the device of p");
+    TORCH_CHECK(anchor_rows.has_value() && anchor_rows->defined(), who, ": a prox anchor needs anchor_rows");
+    const Tensor& ar = *anchor_rows;
+    TORCH_CHECK(ar.is_cuda() && ar.device() == p.device() && ar.scalar_type() == torch::kInt32 && ar.is_contiguous() && ar.numel() == R,
+                who, ": anchor_rows must be a contiguous int32 [R] tensor on the device of p");
+    // the entries of anchor_rows are not range-checked here: reading them would synchronise (and break CUDA-graph capture);
+    // the engine builds them from slot indices < A
+    px.mu = (float)mu; px.anchor = a.data_ptr<float>(); px.astride = a.stride(0); px.rows = ar.data_ptr<int>();
+    if (prox_mask.has_value() && prox_mask->defined()) {
+        const Tensor& mk = *prox_mask;
+        TORCH_CHECK(mk.is_cuda() && mk.device() == p.device() && mk.scalar_type() == torch::kUInt8 && mk.is_contiguous() && mk.numel() >= P,
+                    who, ": the prox mask must be a contiguous uint8 [>= P] tensor on the device of p");
+        px.mask = mk.data_ptr<unsigned char>();
+    }
+    return px;
+}
+
 void adam_amsgrad_rows(Tensor p, Tensor g, Tensor m, Tensor v, Tensor vmax, Tensor steps, double lr, double wd, double b1, double b2, double eps,
-                       c10::optional<Tensor> row_mask) {
+                       c10::optional<Tensor> row_mask, double prox_mu, c10::optional<Tensor> anchor, c10::optional<Tensor> anchor_rows,
+                       c10::optional<Tensor> prox_mask) {
     CHECK_CUDA_F32(p); CHECK_CUDA_F32(g); CHECK_CUDA_F32(m); CHECK_CUDA_F32(v); CHECK_CUDA_F32(vmax); CHECK_CUDA_I32(steps);
     c10::cuda::CUDAGuard guard(p.device());
     TORCH_CHECK(p.is_contiguous() && m.is_contiguous() && v.is_contiguous() && vmax.is_contiguous(), "arena rows must be contiguous");
     const int R = (int)steps.numel();
     const long long P = p.numel() / R;
+    const fdb::ProxAnchor px = prox_anchor("adam_amsgrad_rows", p, R, P, prox_mu, anchor, anchor_rows, prox_mask);
+    TORCH_CHECK(px.anchor == nullptr || (g.is_contiguous() && g.numel() == p.numel()),
+                "adam_amsgrad_rows: with a prox anchor g must be contiguous like p (it receives the effective gradient)");
     CHECK_OK(fdb::adam_amsgrad_rows_launch(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
                                            vmax.data_ptr<float>(), steps.data_ptr<int>(), opt_ptr<unsigned char>(row_mask), R, P, (float)lr,
-                                           (float)wd, (float)b1, (float)b2, (float)eps, cur_stream()), "adam_amsgrad_rows");
+                                           (float)wd, (float)b1, (float)b2, (float)eps, px, cur_stream()), "adam_amsgrad_rows");
 }
-void sgd_rows(Tensor p, Tensor g, double lr, double wd) {
+// without row mask and anchor: one flat pass over p; otherwise p is [R, P] rows (row_mask uint8 [R] skips rows)
+void sgd_rows(Tensor p, Tensor g, double lr, double wd, c10::optional<Tensor> row_mask, double prox_mu, c10::optional<Tensor> anchor,
+              c10::optional<Tensor> anchor_rows, c10::optional<Tensor> prox_mask) {
     CHECK_CUDA_F32(p); CHECK_CUDA_F32(g);
     c10::cuda::CUDAGuard guard(p.device());
-    CHECK_OK(fdb::sgd_rows_launch(p.data_ptr<float>(), g.data_ptr<float>(), p.numel(), (float)lr, (float)wd, cur_stream()), "sgd_rows");
+    const bool has_mask = row_mask.has_value() && row_mask->defined(), has_anchor = anchor.has_value() && anchor->defined();
+    if (!has_mask && !has_anchor) {
+        CHECK_OK(fdb::sgd_rows_launch(p.data_ptr<float>(), g.data_ptr<float>(), p.numel(), (float)lr, (float)wd, cur_stream()), "sgd_rows");
+        return;
+    }
+    TORCH_CHECK(p.dim() == 2 && p.is_contiguous() && g.sizes() == p.sizes() && g.is_contiguous(),
+                "sgd_rows: with a row mask or prox anchor, p and g must be contiguous [R, P] tensors");
+    const int64_t R = p.size(0), P = p.size(1);
+    TORCH_CHECK(R <= 65535, "sgd_rows: at most 65535 rows (one grid row each)");
+    if (has_mask)
+        TORCH_CHECK(row_mask->is_cuda() && row_mask->device() == p.device() && row_mask->scalar_type() == torch::kUInt8 &&
+                        row_mask->is_contiguous() && row_mask->numel() == R, "sgd_rows: row_mask must be a contiguous uint8 [R] tensor");
+    const fdb::ProxAnchor px = prox_anchor("sgd_rows", p, R, P, prox_mu, anchor, anchor_rows, prox_mask);
+    if (R == 0 || P == 0) return;
+    CHECK_OK(fdb::sgd_rows_masked_launch(p.data_ptr<float>(), g.data_ptr<float>(), opt_ptr<unsigned char>(row_mask), (int)R, P, (float)lr,
+                                         (float)wd, px, cur_stream()), "sgd_rows");
 }
 
 // ---------------------------------------------------------------------------------- clustering geometry / MPC / misc

@@ -88,8 +88,8 @@ struct BatchSel {
 };
 
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
-// its code and register allocation
-template <class Net, bool kDefend>
+// its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0), separate for the same reason
+template <class Net, bool kDefend, bool kProx>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P, IN = Net::kIn, OUT = Net::kOut, HID = Net::kHid;
@@ -388,6 +388,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                             float gs = gcol[q];
                             for (int w2 = 1; w2 < WPP; ++w2) gs += wsum[w2 * P + pp];
                             float w = thl[pp];
+                            // FedProx: θ_s still holds the round-start models during local training
+                            if constexpr (kProx) gs = fmaf(p.prox_mu, w - theta_s[m * P + pp], gs);
                             if (p.use_adam) {
                                 gs = fmaf(p.wd, w, gs);
                                 om[q] = fmaf(gs - om[q], 1.0f - b1, om[q]);
@@ -739,7 +741,9 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     const SmemLayout L = make_layout<Net>(p.M, p.C, pairs_per_cta, p.sopt_kind != 0);
     const int smem = L.total * (int)sizeof(float);
     if (smem > 227 * 1024) return -2;
-    auto kern = p.def_bound > 0.f ? fed_round_small_kernel<Net, true> : fed_round_small_kernel<Net, false>;
+    const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f;
+    auto kern = prox ? (defend ? fed_round_small_kernel<Net, true, true> : fed_round_small_kernel<Net, false, true>)
+                     : (defend ? fed_round_small_kernel<Net, true, false> : fed_round_small_kernel<Net, false, false>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return -3;
     cudaLaunchConfig_t cfg{};

@@ -37,7 +37,9 @@ struct RoundParams {
     // robust aggregation (def_bound 0 = off): each pair's upload x enters its slot's average as θ_m + s·(x − θ_m),
     // s = 1 / max(1, ‖x − θ_m‖ / def_bound), plus def_stddev·gauss_hash(defense_seed(seed, round), c·M + m, e) (weak DP)
     float def_bound, def_stddev;
-    float* client_out;   // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
+    // FedProx (0 = off): every local step of pair (c, m) adds prox_mu·(w − θ_m) to the gradient, θ_m the round-start model
+    float prox_mu;
+    float* client_out;  // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs
     float* metrics;      // [rounds, C, 4]

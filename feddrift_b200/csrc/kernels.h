@@ -31,9 +31,22 @@ int aue_sqerr_launch(const float* logits, const int* target, int B, int K, float
 int ensemble_vote_launch(const int* preds, const float* w, int Kmodels, int B, int classes, int* out, cudaStream_t stream);
 int confusion_matrix_launch(const int* pred, const int* target, int B, int classes, int* out, cudaStream_t stream);
 // optim.cu
-int adam_amsgrad_rows_launch(float* p, const float* g, float* m, float* v, float* vmax, int* steps, const unsigned char* row_mask, int R,
-                             long long P, float lr, float wd, float b1, float b2, float eps, cudaStream_t stream);
+// FedProx anchor of the row optimizers (anchor == nullptr: off): row r's gradient becomes g + mu·mask⊙(w − anchor row
+// rows[r]); anchor is [A, astride ≥ P] with unit column stride, mask a [P] uint8 entry mask or nullptr (every entry)
+struct ProxAnchor {
+    float mu;
+    const float* anchor;
+    long long astride;
+    const int* rows;
+    const unsigned char* mask;
+};
+// with a prox anchor, g is overwritten by the effective gradient
+int adam_amsgrad_rows_launch(float* p, float* g, float* m, float* v, float* vmax, int* steps, const unsigned char* row_mask, int R,
+                             long long P, float lr, float wd, float b1, float b2, float eps, const ProxAnchor& prox, cudaStream_t stream);
 int sgd_rows_launch(float* p, const float* g, long long n, float lr, float wd, cudaStream_t stream);
+// rows [R, P]: rows with row_mask[r] == 0 are skipped
+int sgd_rows_masked_launch(float* p, const float* g, const unsigned char* row_mask, int R, long long P, float lr, float wd,
+                           const ProxAnchor& prox, cudaStream_t stream);
 // cluster_ops.cu
 long long gram_workspace_doubles();
 int gram_launch(const float* U, int n, long long P, double eps, double* S, double* nrm, double* part, cudaStream_t stream);

@@ -34,6 +34,7 @@ from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
 from ..core.robustness import make_defense
+from ..ops.reference import prox_mu_param
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
@@ -248,6 +249,7 @@ class FedAvgEnsTrainer:
         self.criterions = [nn.CrossEntropyLoss().to(device) for _ in models]
         self.optimizers = [self._make_optimizer(m) for m in models]
         self.rng = np.random.RandomState(int(getattr(args, "dummy_arg", 0)) * 1000 + int(client_index) + 1)
+        self.fedprox_mu = prox_mu_param(getattr(args, "fedprox_mu", 0.0))
 
     def _make_optimizer(self, m):
         if self.args.client_optimizer == "sgd":
@@ -296,12 +298,17 @@ class FedAvgEnsTrainer:
             model.train()
             self._before_train(mod_idx)
             opt, crit = self.optimizers[mod_idx], self.criterions[mod_idx]
+            # FedProx (--fedprox_mu): the local objective gains mu/2‖w − w0‖² over the trainable parameters, w0 = the received model
+            prox = [(p, p.detach().clone()) for p in model.parameters() if p.requires_grad] if self.fedprox_mu > 0 else []
             for _ in range(self.args.epochs):
                 x, labels = sampler()
                 x, labels = self._transform(mod_idx, x.to(self.device)), labels.to(self.device)
                 opt.zero_grad()
                 loss = crit(model(x), labels)
                 loss.backward()
+                for p, p0 in prox:
+                    if p.grad is not None:
+                        p.grad.add_(p.detach() - p0, alpha=self.fedprox_mu)
                 opt.step()
             weights = {k: v.detach().cpu() for k, v in model.state_dict().items()}
             if getattr(self.args, "is_mobile", 0) == 1:

@@ -25,6 +25,11 @@ CONFIGS = {
                                                      concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
                                                      concept_num=4, change_points="A", sample_num=100, batch_size=500,
                                                      comm_round=40, defense_type="weak_dp", norm_bound=5.0, stddev=0.025),
+    # config 2 with FedProx local training: every local step adds 0.1·(w − θ_m) to the gradient, θ_m the received cluster model
+    "cfg2x_sea_fnn_100clients_fedprox_feddrift": dict(model="fnn", dataset="sea", client_num_in_total=100, client_num_per_round=100,
+                                                      concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
+                                                      concept_num=4, change_points="A", sample_num=100, batch_size=500,
+                                                      comm_round=40, fedprox_mu=0.1),
     # config 3: MNIST 2-conv CNN, 4 concepts, 64 clients, IFCA hard-r
     "cfg3_mnist_cnn_64clients_ifca": dict(model="cnn", dataset="MNIST", client_num_in_total=64, client_num_per_round=64,
                                           concept_drift_algo="softclusterwin-1", concept_drift_algo_arg="hard-r", concept_num=4,

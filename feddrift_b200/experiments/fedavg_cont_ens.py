@@ -58,6 +58,8 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     # the reference's backdoor defense (clipping + Gaussian noise) and carries no (ε, δ) privacy guarantee
     a("--defense_type", type=str, default="none", choices=["none", "norm_diff_clipping", "weak_dp"])
     a("--norm_bound", type=float, default=5.0); a("--stddev", type=float, default=0.025, help="weak_dp noise stddev")
+    # FedProx local training: every client step minimises CE + mu/2‖w − w_m‖², w_m the cluster model it received (0 = off)
+    a("--fedprox_mu", type=float, default=0.0)
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)
     a("--pack_workers", type=int, default=0); a("--zero_copy", type=int, default=0)
     a("--round_timeout_s", type=float, default=0.0, help="> 0: close a round without workers whose upload did not arrive in time")

@@ -172,24 +172,45 @@ def gram_cosine(U, eps: float = 1e-12):
 
 
 # ----------------------------------------------------------------------------- arena optimizer
-def adam_amsgrad_rows_(p, g, m, v, vmax, steps, lr: float, wd: float, b1=0.9, b2=0.999, eps=1e-8, row_mask=None):
-    """Fused Adam(amsgrad, L2 wd) over arena rows [R,P]; ``steps`` [R] int32 is incremented in place."""
+def _prox_args(prox):
+    """``prox=(mu, anchor, anchor_rows, mask)`` → the trailing arguments of the native row optimizers (no anchor: off)."""
+    if prox is None:
+        return 0.0, None, None, None
+    mu, anchor, rows, mask = prox
+    return float(mu), anchor, rows, mask
+
+
+def adam_amsgrad_rows_(p, g, m, v, vmax, steps, lr: float, wd: float, b1=0.9, b2=0.999, eps=1e-8, row_mask=None, prox=None):
+    """Fused Adam(amsgrad, L2 wd) over arena rows [R,P]; ``steps`` [R] int32 is incremented in place.  ``prox=(mu, anchor,
+    anchor_rows, mask)`` adds the FedProx term mu·mask⊙(p[r] − anchor[anchor_rows[r]]) to row r's gradient before the wd term
+    (``reference.prox_grad``): anchor [A, ≥ P] with unit column stride, anchor_rows int32 [R], mask uint8 [P] or None.  With
+    ``prox``, the updated rows of ``g`` are overwritten by that effective gradient (g must be contiguous)."""
     if native(p):
-        _ext.load().adam_amsgrad_rows(p, g.contiguous(), m, v, vmax, steps, float(lr), float(wd), float(b1),
-                                      float(b2), float(eps), row_mask)
+        _ext.load().adam_amsgrad_rows(p, g if prox is not None else g.contiguous(), m, v, vmax, steps, float(lr), float(wd), float(b1),
+                                      float(b2), float(eps), row_mask, *_prox_args(prox))
         return p
     for r in range(p.shape[0]):
         if row_mask is not None and not bool(row_mask[r]):
             continue
+        if prox is not None:
+            g[r] = ref.prox_grad(g[r], p[r], prox, r)
         steps[r] = ref.adam_amsgrad_update(p[r], g[r], m[r], v[r], vmax[r], int(steps[r]), lr, wd, b1, b2, eps)
     return p
 
 
-def sgd_rows_(p, g, lr: float, wd: float = 0.0):
+def sgd_rows_(p, g, lr: float, wd: float = 0.0, row_mask=None, prox=None):
+    """p ← p − lr·(g + wd·p) over arena rows [R,P]; ``row_mask`` uint8 [R] skips rows, ``prox`` as in ``adam_amsgrad_rows_``."""
     if native(p):
-        _ext.load().sgd_rows(p, g.contiguous(), float(lr), float(wd))
+        _ext.load().sgd_rows(p, g.contiguous(), float(lr), float(wd), row_mask, *_prox_args(prox))
         return p
-    p.add_(g + wd * p, alpha=-lr)
+    if row_mask is None and prox is None:
+        p.add_(g + wd * p, alpha=-lr)
+        return p
+    for r in range(p.shape[0]):
+        if row_mask is not None and not bool(row_mask[r]):
+            continue
+        gr = g[r] if prox is None else ref.prox_grad(g[r], p[r], prox, r)
+        p[r].add_(gr + wd * p[r], alpha=-lr)
     return p
 
 

@@ -91,6 +91,19 @@ def adam_amsgrad_update(p, g, m, v, vmax, step: int, lr, wd, b1=0.9, b2=0.999, e
     return step
 
 
+def prox_grad(g, w, prox, r: int = 0):
+    """FedProx (``--fedprox_mu``): the gradient of F(w) + μ/2‖mask ⊙ (w − a)‖², i.e. g + μ·mask ⊙ (w − a), for row r of a
+    row optimizer; ``prox = (mu, anchor, anchor_rows, mask)``, a = anchor[anchor_rows[r], :P] (anchor_rows None: anchor is the
+    row itself), mask a [≥ P] entry mask or None (every entry)."""
+    mu, anchor, rows, mask = prox
+    P = w.shape[-1]
+    a = anchor if rows is None else anchor[int(rows[r])]
+    d = w - a[:P]
+    if mask is not None:
+        d = d * mask[:P].to(d.dtype)
+    return g + float(mu) * d
+
+
 def mlp_eval(theta, x, y, n, kind, din, hid, dout) -> Tuple[float, float]:
     """-> (correct, loss_sum) over the first n samples."""
     if n == 0:
@@ -199,7 +212,9 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     ``defense`` 'norm_diff_clipping'|'weak_dp' (absent or 'none': off) with ``norm_bound`` (5.0) and ``stddev`` (0.025, weak_dp
     only): before the average, every trained pair's local model goes through ``robust_clip_slots_`` against the round-start θ
     with seed ``defense_seed(seed, rnd)``; the weights are unchanged.  ``client_out [C, M, P]``: the raw (undefended) local
-    models of the pairs that trained in the last round are written there.
+    models of the pairs that trained in the last round are written there.  ``fedprox_mu`` (absent or 0: off): every local
+    step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
+    (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
     Mutates theta / opt state / W (if recluster) in place; returns ``metrics [rounds, C, 4]`` =
     (train_correct, train_loss_sum, test_correct, test_loss_sum) and ``counts [C, 2]`` = (n_train, n_test).
     """
@@ -224,6 +239,7 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
         sopt = None
     defense = st.get("defense") or "none"
     def_bound, def_std = defense_params(defense, st.get("norm_bound", 5.0), st.get("stddev", 0.025))
+    prox_mu = prox_mu_param(st.get("fedprox_mu", 0.0))
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -255,6 +271,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                     if feat_mask is not None:
                         xb = xb * feat_mask[m]
                     _, g = mlp_loss_grad(p, xb, yb, kind, din, hid, dout)
+                    if prox_mu > 0:
+                        g = prox_grad(g, p, (prox_mu, theta[m], None, None))
                     if use_adam:
                         st["opt_step"][c, m] = adam_amsgrad_update(
                             p, g, st["opt_m"][c, m], st["opt_v"][c, m], st["opt_vmax"][c, m],
@@ -406,6 +424,14 @@ def defense_params(defense: str, norm_bound: float, stddev: float) -> Tuple[floa
     if not math.isfinite(std) or std < 0.0:
         raise ValueError(f"stddev must be finite and >= 0 (got {stddev!r})")
     return bound, (std if defense == "weak_dp" else 0.0)
+
+
+def prox_mu_param(mu) -> float:
+    """Validated FedProx coefficient (``--fedprox_mu``): a finite float ≥ 0, else ``ValueError``."""
+    mu = float(mu)
+    if not math.isfinite(mu) or mu < 0:
+        raise ValueError(f"fedprox_mu must be finite and >= 0 (got {mu})")
+    return mu
 
 
 def defense_seed(seed: int, rnd: int) -> int:

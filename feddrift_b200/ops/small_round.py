@@ -136,6 +136,10 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         if len(fcfg) == 5:
             fcfg += [1.0, 0.0, 1e-8]   # server optimizer slots, unread without one
         fcfg += list(defense_params(defense, st.get("norm_bound", 5.0), st.get("stddev", 0.025)))
+    prox_mu = float(st.get("fedprox_mu", 0.0) or 0.0)
+    if prox_mu != 0.0:   # FedProx in every local step; the binding validates mu
+        fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer / defense slots, unread when off
+        fcfg.append(prox_mu)
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out

@@ -36,6 +36,7 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
+from ..ops.reference import prox_mu_param
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -50,7 +51,7 @@ DEFAULTS = dict(
     change_points="A", time_stretch=1, reset_models=0, noise_prob=0.0, dummy_arg=0, sample_num=100, ci=0,
     is_mobile=0, gpu_num_per_server=1, data_dir=None, checkpoint_dir=None, rounds_per_launch=0,
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
-    defense_type="none", norm_bound=5.0, stddev=0.025,
+    defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
 )
 
 
@@ -96,6 +97,10 @@ class DriftSim:
         # robust aggregation (--defense_type): uploads are clipped (+ noised) against the round-start models before averaging
         self.defense = make_defense(args)
         self.defense_mask = None if bool(wmask[: self.bank.P].all()) else wmask[: self.bank.P].to(self.device)
+        # FedProx (--fedprox_mu): every local step adds mu·mask⊙(w − θ_m) to the gradient, θ_m the round-start model; the
+        # generic routes take the trainable-entry mask as uint8 (BatchNorm statistics get no proximal term)
+        self.fedprox_mu = prox_mu_param(getattr(args, "fedprox_mu", 0.0))
+        self.prox_mask = None if self.defense_mask is None else self.defense_mask.to(torch.uint8)
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -213,6 +218,8 @@ class DriftSim:
                                    server_s0=so.s0, server_s1=so.s1, server_step=so.step)
             if self.defense is not None:
                 self._small.update(defense=self.defense.defense_type, norm_bound=self.defense.norm_bound, stddev=self.defense.stddev)
+            if self.fedprox_mu > 0:
+                self._small["fedprox_mu"] = self.fedprox_mu
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)

@@ -213,6 +213,11 @@ class _GraphedStep:
         z = lambda: torch.zeros(P, dtype=torch.float32, device=dev)  # noqa: E731
         self.row, self.g, self.m, self.v, self.vmax = z(), z(), z(), z(), z()
         self.step = torch.zeros(1, dtype=torch.int32, device=dev)
+        # FedProx: the pair's start row (its round-start cluster model), filled by load(); anchor table [0]
+        self.mu = float(sim.fedprox_mu)
+        self.anchor = z() if self.mu > 0 else None
+        self.prox = (self.mu, self.anchor.view(1, -1), torch.zeros(1, dtype=torch.int32, device=dev), sim.prox_mask) \
+            if self.mu > 0 else None
         self.x = torch.zeros(batch_shape, dtype=sim.data.X.dtype, device=dev)
         self.y = torch.zeros(batch_shape[0], dtype=torch.long, device=dev)
         self.steps, self.indexed = int(steps), bool(indexed)
@@ -254,9 +259,9 @@ class _GraphedStep:
             F.cross_entropy(self.mod(x), y).backward()
             if self.use_adam:
                 ops.adam_amsgrad_rows_(self.row.view(1, -1), self.g.view(1, -1), self.m.view(1, -1), self.v.view(1, -1),
-                                       self.vmax.view(1, -1), self.step, self.lr, self.wd)
+                                       self.vmax.view(1, -1), self.step, self.lr, self.wd, prox=self.prox)
             else:
-                ops.sgd_rows_(self.row.view(1, -1), self.g.view(1, -1), self.lr, 0.0)
+                ops.sgd_rows_(self.row.view(1, -1), self.g.view(1, -1), self.lr, 0.0, prox=self.prox)
 
     def load(self, cl, c, m):
         if self.use_adam:   # one multi-tensor copy kernel instead of four
@@ -264,6 +269,8 @@ class _GraphedStep:
             self.step.copy_(cl.step[c, m].reshape(1))
         else:
             self.row.copy_(cl.params[c, m])
+        if self.anchor is not None:
+            self.anchor.copy_(self.row)
 
     def store(self, cl, c, m):
         if self.use_adam:
@@ -311,12 +318,12 @@ def _join_slots(sim, slots):
 
 
 def _graphed_step(sim, batch_shape, use_adam, lr, wd, slot: int = 0, steps: int = 1, indexed: bool = False):
-    """Cached ``_GraphedStep`` for this (batch shape, optimizer, lr) or None when graphs are unavailable."""
+    """Cached ``_GraphedStep`` for this (batch shape, optimizer, lr, FedProx mu) or None when graphs are unavailable."""
     if sim.device.type != "cuda" or sim.bank.mlp is not None or os.environ.get("FDB_NO_GRAPHS") == "1" \
             or getattr(sim, "_graphs_broken", False):
         return None
     cache = sim.__dict__.setdefault("_step_graphs", {})
-    key = (tuple(batch_shape), bool(use_adam), float(lr), float(wd), int(slot), int(steps), bool(indexed))
+    key = (tuple(batch_shape), bool(use_adam), float(lr), float(wd), int(slot), int(steps), bool(indexed), float(sim.fedprox_mu))
     gs = cache.get(key)
     if gs is None:
         nslots = max(1, len(sim.__dict__.get("_slot_streams") or [1]))
@@ -383,6 +390,7 @@ def _local_steps(sim, c, m, xy, sampler, seed, rnd, E, use_adam, lr, wd, feat_ma
         mod = _scratch_module(sim)
         _bind(mod, bank, row)
         mod.train()
+    prox = _prox(sim, m)
     for xb, yb in batches:
         if mlp is not None:
             th = row.detach().clone().requires_grad_(True)
@@ -396,9 +404,19 @@ def _local_steps(sim, c, m, xy, sampler, seed, rnd, E, use_adam, lr, wd, feat_ma
         r2 = row.reshape(1, -1)
         if use_adam:
             ops.adam_amsgrad_rows_(r2, g.reshape(1, -1), cl.m[c, m].reshape(1, -1), cl.v[c, m].reshape(1, -1),
-                                   cl.vmax[c, m].reshape(1, -1), cl.step[c, m].reshape(1), lr, wd)
+                                   cl.vmax[c, m].reshape(1, -1), cl.step[c, m].reshape(1), lr, wd, prox=prox)
         else:
-            ops.sgd_rows_(r2, g.reshape(1, -1), lr, 0.0)
+            ops.sgd_rows_(r2, g.reshape(1, -1), lr, 0.0, prox=prox)
+
+
+def _prox(sim, m: int):
+    """FedProx anchor of a pair of slot m on the eager paths: the slot's round-start model ``bank.theta[m]`` (None: off)."""
+    if sim.fedprox_mu <= 0:
+        return None
+    zero = sim.__dict__.get("_prox_row0")
+    if zero is None or zero.device != sim.device:
+        zero = sim._prox_row0 = torch.zeros(1, dtype=torch.int32, device=sim.device)
+    return sim.fedprox_mu, sim.bank.theta[m:m + 1], zero, sim.prox_mask
 
 
 def _scratch_module(sim):

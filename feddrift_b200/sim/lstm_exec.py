@@ -115,6 +115,10 @@ def train_pairs(sim, pairs: List, seed: int, rnd: int, E: int, use_adam: bool, l
     ext = _ext.load(required=True)
     o_emb, n_emb, _ = lay["emb"]
     o_wih1 = lay["w_ih1"][0]
+    prox = None
+    if sim.fedprox_mu > 0:   # FedProx: arena row r = c·M + m is anchored at its slot's round-start model, bank row r % M
+        arows = torch.arange(C * M, dtype=torch.int32, device=dev) % M
+        prox = (sim.fedprox_mu, bank.theta, arows, sim.prox_mask)
 
     def put(name: str, t: torch.Tensor) -> None:                         # per-pair gradient block → its slot in the gradient rows
         off, n, _ = lay[name]
@@ -136,6 +140,8 @@ def train_pairs(sim, pairs: List, seed: int, rnd: int, E: int, use_adam: bool, l
         put("w_ih1", dWih1); put("emb", demb); put("fc_w", dWfc); put("fc_b", dbfc)
         if use_adam:
             ops.adam_amsgrad_rows_(params2, G, cl.m.view(C * M, P), cl.v.view(C * M, P), cl.vmax.view(C * M, P), cl.step.view(-1),
-                                   lr, wd, row_mask=mask)
-        else:
+                                   lr, wd, row_mask=mask, prox=prox)
+        elif prox is not None and e > 0:
+            ops.sgd_rows_(params2, G, lr, 0.0, row_mask=mask, prox=prox)
+        else:   # also FedProx's first step: every pair sits at its anchor there, so the proximal term is 0
             params2.index_add_(0, rows, G.index_select(0, rows), alpha=-lr)

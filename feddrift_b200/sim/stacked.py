@@ -363,6 +363,8 @@ def _train_pass(sim, pairs: List, seed: int, rnd: int, E: int, use_adam: bool, l
     Xf = sim.data.X.reshape(-1, *sim.data.X.shape[3:])
     Yf = sim.data.Y.reshape(-1)
     tmpl = bank.template
+    # FedProx: pair i's anchor is its slot's round-start model, bank row ms[i]
+    prox = (sim.fedprox_mu, bank.theta, ms.to(torch.int32), sim.prox_mask) if sim.fedprox_mu > 0 else None
 
     for e in range(E):
         x = Xf[gidx[e]]                                                       # [npairs, B, *features]
@@ -374,9 +376,9 @@ def _train_pass(sim, pairs: List, seed: int, rnd: int, E: int, use_adam: bool, l
         loss = F.cross_entropy(logits.reshape(B * npairs, K), y.t().reshape(-1), reduction="sum") / B
         loss.backward()
         if use_adam:
-            ops.adam_amsgrad_rows_(st.params, st.grads, st.m, st.v, st.vmax, st.step, lr, wd)
+            ops.adam_amsgrad_rows_(st.params, st.grads, st.m, st.v, st.vmax, st.step, lr, wd, prox=prox)
         else:
-            ops.sgd_rows_(st.params, st.grads, lr, 0.0)
+            ops.sgd_rows_(st.params, st.grads, lr, 0.0, prox=prox)
     st.store_buffers()
     cl.params.view(CM, P).index_copy_(0, rows, st.params)
     if use_adam:
