@@ -131,6 +131,13 @@ std::vector<int64_t> fed_round_small(
         p.prox_mu = (float)fcfg[10];
         TORCH_CHECK(std::isfinite(p.prox_mu), "fed_round_small: fedprox_mu overflows float32");
     }
+    if (fcfg.size() >= 13) {   // QSGD upload compression: fcfg[11] = level s (0 = off), fcfg[12] = bucket size b
+        const double s = fcfg[11], b = fcfg[12];
+        TORCH_CHECK(s == std::floor(s) && s >= 0.0 && s <= 65535.0, "fed_round_small: quantize_level must be an integer in [1, 65535] (0 = off)");
+        TORCH_CHECK(s == 0.0 || (b == std::floor(b) && b >= 1.0 && b <= 2147483647.0),
+                    "fed_round_small: quantize_bucket must be an integer >= 1");
+        p.q_level = (int)s; p.q_bucket = s == 0.0 ? 0 : (int)b;
+    }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
     TORCH_CHECK(rc != -1, "fed_round_small: MLP shape (", kind, ",", din, ",", hid, ",", dout, ") is not instantiated");
@@ -301,6 +308,42 @@ Tensor robust_clip_slots(Tensor rows, Tensor theta, c10::optional<Tensor> n, dou
                                      (float)bound, scratch.data_ptr<float>(), nrm.data_ptr<float>(), (float)stddev, (unsigned)seed,
                                      cur_stream()), "robust_clip_slots");
     return nrm;
+}
+
+// K17 over an upload arena rows [C, M, P] (contiguous), in place: row (c, m) with n[c, m] > 0 (every row when n is None) is
+// QSGD-quantized against its slot's model theta[m, :P] (theta [M, stride >= P], unit column stride, e.g. a padded ModelBank)
+// with level s and bucket b; entries whose mask byte is 0 pass through.  The draws are uniform_hash(seed, c·M + m, e).
+void qsgd_slots(Tensor rows, Tensor theta, c10::optional<Tensor> n, int64_t level, int64_t bucket, c10::optional<Tensor> mask,
+                int64_t seed) {
+    CHECK_CUDA_F32(rows); CHECK_CUDA_F32(theta);
+    TORCH_CHECK(rows.is_contiguous() && rows.dim() == 3, "qsgd_slots: rows must be a contiguous [C, M, P] tensor");
+    const int64_t M = rows.size(1), P = rows.size(2), R = rows.size(0) * M;
+    TORCH_CHECK(M >= 1 && R <= 65535, "qsgd_slots: need M >= 1 and at most 65535 rows (one grid row each)");
+    TORCH_CHECK(P < (int64_t(1) << 31), "qsgd_slots: rows of 2^31 or more entries are not supported");
+    TORCH_CHECK(theta.device() == rows.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "qsgd_slots: theta must be [M, >= P] with unit column stride on the device of rows");
+    TORCH_CHECK(level >= 1 && level <= 65535, "qsgd_slots: level must be in [1, 65535]");
+    TORCH_CHECK(bucket >= 1, "qsgd_slots: bucket must be >= 1");
+    TORCH_CHECK(seed >= 0 && seed <= 0xFFFFFFFFLL, "qsgd_slots: seed must be a 32-bit unsigned value");
+    const float* np_ = nullptr;
+    if (n.has_value() && n->defined()) {
+        TORCH_CHECK(n->is_cuda() && n->device() == rows.device() && n->scalar_type() == torch::kFloat32 && n->is_contiguous() &&
+                    n->numel() == R, "qsgd_slots: n must be a contiguous float32 [C, M] tensor on the device of rows");
+        np_ = n->data_ptr<float>();
+    }
+    const unsigned char* mp = nullptr;
+    if (mask.has_value() && mask->defined()) {
+        TORCH_CHECK(mask->is_cuda() && mask->device() == rows.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                    mask->numel() >= P, "qsgd_slots: mask must be a contiguous uint8 [>= P] tensor on the device of rows");
+        mp = mask->data_ptr<unsigned char>();
+    }
+    if (R == 0 || P == 0) return;
+    c10::cuda::CUDAGuard guard(rows.device());
+    const int64_t b = std::min<int64_t>(bucket, P), nb = (P + b - 1) / b;
+    auto scratch = torch::empty({R * nb}, rows.options().dtype(torch::kInt32));
+    CHECK_OK(fdb::qsgd_slots_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)M, np_, mp, (int)R, P,
+                                    (int)level, b, reinterpret_cast<unsigned*>(scratch.data_ptr<int>()), (unsigned)seed, cur_stream()),
+             "qsgd_slots");
 }
 
 // cp: the client arena [C_arena, M, P]; cidx: int32 [C] arena rows of this rank's clients (or None: rows 0..C-1 of cp);
@@ -948,6 +991,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("gossip_mix", &gossip_mix);
     m.def("robust_clip", &robust_clip);
     m.def("robust_clip_slots", &robust_clip_slots);
+    m.def("qsgd_slots", &qsgd_slots);
     m.def("eval_logits", &eval_logits);
     m.def("aue_sqerr", &aue_sqerr);
     m.def("ensemble_vote", &ensemble_vote);

@@ -33,6 +33,25 @@ FDB_DEVICE float gauss_hash(uint32_t seed, uint32_t r, unsigned long long i) {
 // gauss_hash seed of the weak-DP noise of round `rnd` of a time step whose engine seed is `seed` (ops/reference.py
 // defense_seed); the noise of (client c, slot m) is gauss_hash(defense_seed(seed, rnd), c·M + m, element)
 FDB_HOST_DEVICE uint32_t defense_seed(uint32_t seed, uint32_t rnd) { return mix32(seed ^ mix32(rnd * 0xC2B2AE35u + 0x2545F491u)); }
+// counter-based U[0, 1): (h >> 8)·2⁻²⁴ with h the first lowbias32 hash of gauss_hash for (seed, row, element) — same
+// function as uniform_hash in ops/reference.py
+FDB_HOST_DEVICE float uniform_hash(uint32_t seed, uint32_t r, unsigned long long i) {
+    const uint32_t base = mix32(seed ^ mix32(r * 0x9E3779B9u + 0x7F4A7C15u)) ^ (uint32_t)(i >> 32) * 0x85EBCA6Bu;
+    return (float)(mix32(base ^ ((uint32_t)i * 2u + 1u)) >> 8) * (1.0f / 16777216.0f);
+}
+// uniform_hash seed of the QSGD draws of round `rnd` of a time step whose engine seed is `seed` (ops/reference.py
+// compress_seed); its constants differ from defense_seed's so that quantization draws and weak-DP noise are independent
+FDB_HOST_DEVICE uint32_t compress_seed(uint32_t seed, uint32_t rnd) { return mix32(seed ^ mix32(rnd * 0x27D4EB2Fu + 0x165667B1u)); }
+// QSGD of one trainable entry x with anchor th, bucket scale sigma > 0, level s and uniform draw u (ops/reference.py
+// qsgd_slots_): a = (|d| / σ)·s, q = floor(a) + (u < frac(a)), x' = th + copysign(σ·(q / s), d) with d = x − th.  Every
+// operation is rounded on its own (no FMA contraction), so the result matches the CPU oracle bit for bit.
+FDB_DEVICE float qsgd_entry(float x, float th, float sigma, float s, float u) {
+    const float d = __fsub_rn(x, th);
+    const float a = __fmul_rn(__fdiv_rn(fabsf(d), sigma), s);
+    const float l = floorf(a);
+    const float q = (u < __fsub_rn(a, l)) ? __fadd_rn(l, 1.f) : l;
+    return __fadd_rn(th, copysignf(__fmul_rn(sigma, __fdiv_rn(q, s)), d));
+}
 
 // ---------------------------------------------------------------- warp reductions
 FDB_DEVICE float warp_sum(float v) {

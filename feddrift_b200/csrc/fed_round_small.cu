@@ -88,8 +88,9 @@ struct BatchSel {
 };
 
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
-// its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0), separate for the same reason
-template <class Net, bool kDefend, bool kProx>
+// its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kQuant: the QSGD variant
+// (p.q_level > 0), separate for the same reason
+template <class Net, bool kDefend, bool kProx, bool kQuant>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P, IN = Net::kIn, OUT = Net::kOut, HID = Net::kHid;
@@ -417,6 +418,38 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     }
                     if (lane == 0) p.opt_step[c * M + m] = ostep;
                 }
+                if constexpr (kQuant) {
+                    // QSGD: the client quantizes its update thl − θ_m (θ_s still holds the round-start models) before the
+                    // upload, so client_out, the defense and the average all see the quantized model.  Bucket scales come
+                    // from warp_max over the lane-owned columns, one bucket at a time (P is small, so b < P is cheap).
+                    const int qb = min(p.q_bucket, P);
+                    float sig[COLS];
+#pragma unroll
+                    for (int q = 0; q < COLS; ++q) sig[q] = 0.f;
+                    for (int k0 = 0; k0 < P; k0 += qb) {
+                        float mx = 0.f;
+#pragma unroll
+                        for (int q = 0; q < COLS; ++q) {
+                            const int pp = lane + 32 * q;
+                            if (pp < P && pp >= k0 && pp - k0 < qb) mx = fmaxf(mx, fabsf(thl[pp] - theta_s[m * P + pp]));
+                        }
+                        mx = warp_max(mx);
+#pragma unroll
+                        for (int q = 0; q < COLS; ++q) {
+                            const int pp = lane + 32 * q;
+                            if (pp >= k0 && pp - k0 < qb) sig[q] = mx;
+                        }
+                    }
+                    const uint32_t qseed = compress_seed(p.seed, rnd);
+                    const float qs = (float)p.q_level;
+#pragma unroll
+                    for (int q = 0; q < COLS; ++q) {
+                        const int pp = lane + 32 * q;
+                        if (pp < P && sig[q] > 0.f)
+                            thl[pp] = qsgd_entry(thl[pp], theta_s[m * P + pp], sig[q], qs,
+                                                 uniform_hash(qseed, (uint32_t)k, (unsigned long long)pp));
+                    }
+                }
                 const float wgt = ncm_s[k] / tot_s[m];
                 float dscale = 1.f;
                 bool defend = false;
@@ -444,7 +477,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                                 v = fmaf(p.def_stddev, gauss_hash(defense_seed(p.seed, rnd), (uint32_t)k, (unsigned long long)pp), v);
                         }
                         slot_s[li * P + pp] = v * wgt;
-                        if (p.client_out && r == p.rounds - 1) p.client_out[obase + pp] = thl[pp];   // the raw local model
+                        // the local model as uploaded (quantized under QSGD, before the defense)
+                        if (p.client_out && r == p.rounds - 1) p.client_out[obase + pp] = thl[pp];
                     }
                 }
                 if (lane == 0) slot_model[li] = m;
@@ -725,6 +759,11 @@ __global__ void mlp_eval_matrix_kernel(const float* __restrict__ theta, int thet
 }
 
 // ================================================================================ host launchers
+template <class Net, bool kDefend, bool kProx>
+static auto round_kernel(bool quant) {
+    return quant ? fed_round_small_kernel<Net, kDefend, kProx, true> : fed_round_small_kernel<Net, kDefend, kProx, false>;
+}
+
 template <class Net>
 static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, SmallLaunchInfo* info) {
     using Cfg = SmallCfg<Net>;
@@ -741,9 +780,9 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     const SmemLayout L = make_layout<Net>(p.M, p.C, pairs_per_cta, p.sopt_kind != 0);
     const int smem = L.total * (int)sizeof(float);
     if (smem > 227 * 1024) return -2;
-    const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f;
-    auto kern = prox ? (defend ? fed_round_small_kernel<Net, true, true> : fed_round_small_kernel<Net, false, true>)
-                     : (defend ? fed_round_small_kernel<Net, true, false> : fed_round_small_kernel<Net, false, false>);
+    const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f, quant = p.q_level > 0;
+    auto kern = prox ? (defend ? round_kernel<Net, true, true>(quant) : round_kernel<Net, false, true>(quant))
+                     : (defend ? round_kernel<Net, true, false>(quant) : round_kernel<Net, false, false>(quant));
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return -3;
     cudaLaunchConfig_t cfg{};

@@ -39,6 +39,10 @@ struct RoundParams {
     float def_bound, def_stddev;
     // FedProx (0 = off): every local step of pair (c, m) adds prox_mu·(w − θ_m) to the gradient, θ_m the round-start model
     float prox_mu;
+    // QSGD upload compression (q_level 0 = off): each pair's local model is quantized against θ_m with level q_level and
+    // bucket q_bucket (common.cuh qsgd_entry, draws uniform_hash(compress_seed(seed, round), c·M + m, e)) before client_out,
+    // the defense and the average see it
+    int q_level, q_bucket;
     float* client_out;  // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs

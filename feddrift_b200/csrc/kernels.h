@@ -19,6 +19,10 @@ int gossip_mix_peer_launch(const long long* x_ptrs, const long long* flag_ptrs, 
 // K10: row r of rows [R, P] is clipped around g + (r % M)·g_stride; rows with n[r] == 0 are skipped (n may be nullptr)
 int robust_clip_launch(float* rows, const float* g, long long g_stride, int M, const float* n, const unsigned char* mask, int R,
                        long long P, float bound, float* scratch_nrm2, float* nrm_out, float stddev, unsigned seed, cudaStream_t stream);
+// compress.cu (K17): QSGD of row r of rows [R, P] against theta + (r % M)·t_stride with level s and bucket b; rows with
+// n[r] <= 0 are skipped (n may be nullptr), entries with mask 0 pass through; scratch_smax holds R·⌈P / min(b, P)⌉ words
+int qsgd_slots_launch(float* rows, const float* theta, long long t_stride, int M, const float* n, const unsigned char* mask, int R,
+                      long long P, int level, long long bucket, unsigned* scratch_smax, unsigned seed, cudaStream_t stream);
 // aggregate_peer.cu : multi-GPU reduce-scatter + apply + all-gather over NVLink peer memory (cooperative launch)
 int fedavg_reduce_apply_peer_launch(const float* cp, const int* cidx, const float* n, int C, int M, int P, int theta_stride, int world, int rank,
                                     const long long* part_ptrs, const long long* theta_ptrs, const long long* tot_ptrs,

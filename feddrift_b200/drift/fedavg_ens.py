@@ -34,7 +34,7 @@ from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
 from ..core.robustness import make_defense
-from ..ops.reference import prox_mu_param
+from ..ops.reference import compress_seed, compression_params, prox_mu_param
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
@@ -418,6 +418,11 @@ class _BaseAggregator:
         self.defense = make_defense(args) if self.defend_uploads else None
         self.defense_mask = None if bool(wmask.all()) else wmask.to(self.device)
         self._defense_round = 0
+        # upload compression (--compression qsgd): each arriving upload is quantized against bank.theta[m]; its draws follow
+        # this aggregator's round counter, advanced when a round's uploads are complete (packages without the flags: none)
+        self.q_level, self.q_bucket = compression_params(getattr(args, "compression", "none") or "none",
+                                                         getattr(args, "quantize_level", 16), getattr(args, "quantize_bucket", 512))
+        self._compress_round = 0
         self.models = [self.bank.module(i) for i in range(self.bank.num_models)]
         M, P = self.bank.num_models, self.bank.P
         self.upload = torch.zeros(worker_num, M, P, dtype=torch.float32, device=self.device)
@@ -441,6 +446,16 @@ class _BaseAggregator:
                 if getattr(self.args, "is_mobile", 0) == 1:
                     sd = {k: torch.as_tensor(v) for k, v in sd.items()}
                 self.upload[index, m].copy_(mutils.flatten_state_dict(sd).to(self.device))
+        if self.q_level:   # the client quantized before it uploaded: row = worker index · M + m
+            sel = torch.zeros(self.worker_num, self.bank.num_models, dtype=torch.float32)
+            for m, (sd, n) in weights_and_num_samples.items():
+                if sd is not None and n > 0:
+                    sel[index, int(m)] = 1.0
+            if bool(sel.any()):
+                a = self.args
+                seed = int(getattr(a, "dummy_arg", 0)) * 7919 + 13 + 1000003 * int(getattr(a, "curr_train_iteration", 0) or 0)
+                ops.qsgd_slots_(self.upload, self.bank.theta, sel.to(self.device), self.q_level, self.q_bucket, self.defense_mask,
+                                compress_seed(seed, self._compress_round))
         self.flag_client_model_uploaded_dict[index] = True
 
     def check_whether_all_receive(self):
@@ -448,6 +463,7 @@ class _BaseAggregator:
             return False
         for i in range(self.worker_num):
             self.flag_client_model_uploaded_dict[i] = False
+        self._compress_round += 1
         return True
 
     def _aggregate_models(self, model_mask: Optional[np.ndarray] = None):

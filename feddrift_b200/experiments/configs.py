@@ -30,6 +30,11 @@ CONFIGS = {
                                                       concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
                                                       concept_num=4, change_points="A", sample_num=100, batch_size=500,
                                                       comm_round=40, fedprox_mu=0.1),
+    # config 2 with QSGD upload compression: every upload is quantized to 4 levels per sign (512-entry buckets) before averaging
+    "cfg2q_sea_fnn_100clients_qsgd_feddrift": dict(model="fnn", dataset="sea", client_num_in_total=100, client_num_per_round=100,
+                                                   concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
+                                                   concept_num=4, change_points="A", sample_num=100, batch_size=500,
+                                                   comm_round=40, compression="qsgd", quantize_level=4, quantize_bucket=512),
     # config 3: MNIST 2-conv CNN, 4 concepts, 64 clients, IFCA hard-r
     "cfg3_mnist_cnn_64clients_ifca": dict(model="cnn", dataset="MNIST", client_num_in_total=64, client_num_per_round=64,
                                           concept_drift_algo="softclusterwin-1", concept_drift_algo_arg="hard-r", concept_num=4,

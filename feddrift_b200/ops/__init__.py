@@ -17,6 +17,7 @@ Kernel map (SURVEY §2.9 numbering):
   K12 gossip_mix                                  csrc/aggregate.cu
   K13 modp_matmul                                 csrc/mpc.cu
   K14 kd_kl_loss   K15 vfl_bce_grad   K16 group_norm   csrc/misc.cu
+  K17 qsgd_slots_ (upload quantization)           csrc/compress.cu
 """
 from __future__ import annotations
 
@@ -89,6 +90,18 @@ def robust_clip_slots_(rows, theta, n=None, bound: float = 5.0, weight_mask=None
         out = _ext.load().robust_clip_slots(rows, theta, nn, float(bound), mask, float(stddev), int(seed) & 0xFFFFFFFF)
         return out.view(rows.shape[0], rows.shape[1])
     return ref.robust_clip_slots_(rows, theta, n, bound, weight_mask, stddev, seed)
+
+
+def qsgd_slots_(rows, theta, n=None, level: int = 16, bucket: int = 512, weight_mask=None, seed: int = 0):
+    """K17: QSGD of an upload arena ``rows [C, M, P]`` in place: every row with ``n[c, m] > 0`` is quantized against its
+    slot's model ``theta[m, :P]`` (``theta`` may be a padded bank) with level ``level`` and bucket ``bucket``; the draws are
+    ``uniform_hash(seed, c·M + m, ·)``.  See ``reference.qsgd_slots_``; returns ``rows``."""
+    if native(rows, theta):
+        mask = weight_mask[: rows.shape[2]].to(torch.uint8).contiguous() if weight_mask is not None else None
+        nn = n.float().contiguous() if n is not None else None
+        _ext.load().qsgd_slots(rows, theta, nn, int(level), int(bucket), mask, int(seed) & 0xFFFFFFFF)
+        return rows
+    return ref.qsgd_slots_(rows, theta, n, level, bucket, weight_mask, seed)
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, **kw):

@@ -211,8 +211,12 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     slots keep θ, state and counter (see ``server_opt.SlotServerOpt`` for which state rows each optimizer uses).
     ``defense`` 'norm_diff_clipping'|'weak_dp' (absent or 'none': off) with ``norm_bound`` (5.0) and ``stddev`` (0.025, weak_dp
     only): before the average, every trained pair's local model goes through ``robust_clip_slots_`` against the round-start θ
-    with seed ``defense_seed(seed, rnd)``; the weights are unchanged.  ``client_out [C, M, P]``: the raw (undefended) local
-    models of the pairs that trained in the last round are written there.  ``fedprox_mu`` (absent or 0: off): every local
+    with seed ``defense_seed(seed, rnd)``; the weights are unchanged.  ``compression`` 'qsgd' (absent or 'none': off) with
+    ``quantize_level`` s (16) and ``quantize_bucket`` b (512): right after local training, every trained pair's local model
+    goes through ``qsgd_slots_`` against the round-start θ with seed ``compress_seed(seed, rnd)`` (the client quantizes
+    before it uploads), so ``client_out``, the defense and the average see the quantized model.  ``client_out [C, M, P]``:
+    the local models as uploaded (quantized, undefended) of the pairs that trained in the last round are written there.
+    ``fedprox_mu`` (absent or 0: off): every local
     step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
     (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
     Mutates theta / opt state / W (if recluster) in place; returns ``metrics [rounds, C, 4]`` =
@@ -240,6 +244,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     defense = st.get("defense") or "none"
     def_bound, def_std = defense_params(defense, st.get("norm_bound", 5.0), st.get("stddev", 0.025))
     prox_mu = prox_mu_param(st.get("fedprox_mu", 0.0))
+    q_level, q_bucket = compression_params(st.get("compression") or "none", st.get("quantize_level", 16),
+                                           st.get("quantize_bucket", 512))
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -281,8 +287,16 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                         p.add_(g, alpha=-cur_lr)
                 locals_[(c, m)] = (p, n_cm)
                 acc_w[m] += n_cm
-                if client_out is not None and r == rounds - 1:
-                    client_out[c, m] = p
+        if q_level and locals_:   # QSGD: each client quantizes its upload against the round-start θ_m
+            up = torch.zeros(C, M, P, dtype=torch.float32)
+            trained = torch.zeros(C, M)
+            for (c, m), (p, _) in locals_.items():
+                up[c, m], trained[c, m] = p, 1.0
+            qsgd_slots_(up, theta, trained, q_level, q_bucket, None, compress_seed(seed, rnd))
+            locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
+        if client_out is not None and r == rounds - 1:
+            for (c, m), (p, _) in locals_.items():
+                client_out[c, m] = p
         if defense != "none" and locals_:
             up = torch.zeros(C, M, P, dtype=torch.float32)
             for (c, m), (p, _) in locals_.items():
@@ -467,6 +481,114 @@ def robust_clip_slots_(rows: torch.Tensor, theta: torch.Tensor, n=None, bound: f
             new = torch.where(wm, new, row)
         row.copy_(new)
     return norms
+
+
+COMPRESSIONS = ("none", "qsgd")
+
+
+def _int_param(name: str, v) -> int:
+    if isinstance(v, bool):
+        raise ValueError(f"{name} must be an integer (got {v!r})")
+    try:
+        f = float(v)
+    except (TypeError, ValueError):
+        raise ValueError(f"{name} must be an integer (got {v!r})") from None
+    if not math.isfinite(f) or f != int(f):
+        raise ValueError(f"{name} must be an integer (got {v!r})")
+    return int(f)
+
+
+def compression_params(compression: str, quantize_level, quantize_bucket) -> Tuple[int, int]:
+    """Validated ``(level s, bucket b)`` of the upload compression (``--compression`` / ``--quantize_level`` /
+    ``--quantize_bucket``); ``(0, 0)`` for ``none``.  Raises ``ValueError`` for an unknown compression, a level that is not
+    an integer in [1, 65535], or a bucket that is not an integer ≥ 1 (whatever the compression)."""
+    if compression not in COMPRESSIONS:
+        raise ValueError(f"compression must be one of {', '.join(COMPRESSIONS)} (got {compression!r})")
+    s = _int_param("quantize_level", quantize_level)
+    b = _int_param("quantize_bucket", quantize_bucket)
+    if not 1 <= s <= 65535:
+        raise ValueError(f"quantize_level must be in [1, 65535] (got {quantize_level!r})")
+    if b < 1:
+        raise ValueError(f"quantize_bucket must be >= 1 (got {quantize_bucket!r})")
+    return (s, b) if compression == "qsgd" else (0, 0)
+
+
+def compress_seed(seed: int, rnd: int) -> int:
+    """``uniform_hash`` seed of the QSGD draws in round ``rnd`` of a time step whose engine seed is ``seed`` (the
+    ``compress_seed`` of csrc/common.cuh): a function of (seed, round) only, with constants that differ from
+    ``defense_seed`` so that quantization draws and weak-DP noise are independent."""
+    return mix32((seed & M32) ^ mix32((rnd * 0x27D4EB2F + 0x165667B1) & M32))
+
+
+def uniform_hash(seed: int, rows, P: int) -> torch.Tensor:
+    """``[len(rows), P]`` float32 U[0, 1) draws of (seed, row, element): (h >> 8)·2⁻²⁴ with h the first lowbias32 hash of
+    ``gauss_hash`` — bit-compatible with ``uniform_hash`` in csrc/common.cuh (P < 2³²)."""
+    with np.errstate(over="ignore"):
+        i = np.arange(P, dtype=np.uint32)[None, :]
+        r = np.asarray(rows, dtype=np.uint32).reshape(-1, 1)
+        base = _mix32_np(np.uint32(seed & M32) ^ _mix32_np(r * np.uint32(0x9E3779B9) + np.uint32(0x7F4A7C15)))
+        h1 = _mix32_np(base ^ (i * np.uint32(2) + np.uint32(1)))
+    return torch.from_numpy((h1 >> np.uint32(8)).astype(np.float32) * np.float32(1.0 / 16777216.0))
+
+
+def qsgd_slots_(rows: torch.Tensor, theta: torch.Tensor, n=None, level: int = 16, bucket: int = 512, weight_mask=None,
+                seed: int = 0) -> torch.Tensor:
+    """QSGD (K17) over an upload arena ``rows [C, M, P]``, in place.  Row (c, m) with ``n[c, m] > 0`` (every row when ``n``
+    is None) is quantized against θ_m = ``theta[m, :P]``:
+
+    * d = row − θ_m; entries with ``weight_mask`` False pass through and are not used below;
+    * buckets are the flat ranges [k·b, (k+1)·b); σ_k = max |d_e| over the bucket's trainable entries (a max, so GPU and
+      CPU agree bit for bit); a bucket with σ_k == 0 is left unchanged;
+    * a = (|d_e| / σ_k)·s, q = floor(a) + (u < a − floor(a)) with u = ``uniform_hash(seed, c·M + m, e)``;
+    * row_e = θ_e + copysign(σ_k·(q / s), d_e), every operation rounded in fp32.
+
+    E[row] is the raw upload; with s = 1 every update is ternary.  Returns ``rows``."""
+    C, M, P = rows.shape
+    s, b = compression_params("qsgd", level, bucket)
+    if C * M == 0 or P == 0:
+        return rows
+    b = min(b, P)
+    nb = (P + b - 1) // b
+    th = theta[:, :P].to(rows.device)
+    sel = torch.ones(C, M, dtype=torch.bool) if n is None else (n.detach().cpu().reshape(C, M) > 0)
+    wm = None if weight_mask is None else weight_mask[:P].to(rows.device).bool()
+    sf = torch.tensor(float(s), dtype=torch.float32, device=rows.device)
+    for c, m in sel.nonzero().tolist():
+        row = rows[c, m]
+        d = row - th[m]
+        ad = d.abs()
+        if wm is not None:
+            ad = torch.where(wm, ad, torch.zeros_like(ad))
+        sig = F.pad(ad, (0, nb * b - P)).view(nb, b).amax(1).repeat_interleave(b)[:P]
+        a = (ad / sig) * sf
+        lvl = torch.floor(a)
+        u = uniform_hash(seed, [c * M + m], P)[0].to(rows.device)
+        q = torch.where(u < a - lvl, lvl + 1.0, lvl)
+        new = th[m] + torch.copysign(sig * (q / sf), d)
+        keep = sig == 0
+        if wm is not None:
+            keep = keep | ~wm
+        row.copy_(torch.where(keep, row, new))
+    return rows
+
+
+def qsgd_upload_bits(P_train: int, P_other: int, level: int, bucket: int, weight_mask=None) -> int:
+    """Fixed-length code size in bits of one QSGD upload: 32 bits per bucket holding at least one trainable entry, plus
+    1 + ⌈log₂(s+1)⌉ bits (sign and level) per trainable entry, plus 32 bits per non-trainable entry (sent raw).  The
+    buckets are counted from ``weight_mask`` (bool [P_train + P_other]) when given; without it the trainable entries are
+    taken to be contiguous, so ⌈P_train / b⌉ buckets hold them."""
+    s, b = compression_params("qsgd", level, bucket)
+    P_train, P_other = int(P_train), int(P_other)
+    if weight_mask is not None:
+        wm = torch.as_tensor(weight_mask)[: P_train + P_other].bool().cpu()
+        if int(wm.sum()) != P_train:
+            raise ValueError("weight_mask must hold exactly P_train trainable entries")
+        P = P_train + P_other
+        nb = (P + b - 1) // b
+        buckets = int((F.pad(wm.to(torch.uint8), (0, nb * b - P)).view(nb, b).amax(1) > 0).sum()) if P else 0
+    else:
+        buckets = (P_train + b - 1) // b
+    return 32 * buckets + (1 + int(s).bit_length()) * P_train + 32 * P_other
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

@@ -140,6 +140,12 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
     if prox_mu != 0.0:   # FedProx in every local step; the binding validates mu
         fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer / defense slots, unread when off
         fcfg.append(prox_mu)
+    compression = st.get("compression") or "none"
+    if compression != "none":   # QSGD in the publish step (reference.fed_round_small documents the keys)
+        from .reference import compression_params
+        q = compression_params(compression, st.get("quantize_level", 16), st.get("quantize_bucket", 512))
+        fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer / defense / FedProx slots, unread when off
+        fcfg += [float(q[0]), float(q[1])]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out

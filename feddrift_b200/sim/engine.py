@@ -36,7 +36,7 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import prox_mu_param
+from ..ops.reference import compression_params, prox_mu_param, qsgd_upload_bits
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -52,6 +52,7 @@ DEFAULTS = dict(
     is_mobile=0, gpu_num_per_server=1, data_dir=None, checkpoint_dir=None, rounds_per_launch=0,
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
+    compression="none", quantize_level=16, quantize_bucket=512,
 )
 
 
@@ -101,6 +102,10 @@ class DriftSim:
         # generic routes take the trainable-entry mask as uint8 (BatchNorm statistics get no proximal term)
         self.fedprox_mu = prox_mu_param(getattr(args, "fedprox_mu", 0.0))
         self.prox_mask = None if self.defense_mask is None else self.defense_mask.to(torch.uint8)
+        # upload compression (--compression qsgd): every upload is quantized against its round-start model right after local
+        # training; (q_level, q_bucket) = (0, 0) is off
+        self.q_level, self.q_bucket = compression_params(getattr(args, "compression", "none") or "none",
+                                                         getattr(args, "quantize_level", 16), getattr(args, "quantize_bucket", 512))
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -172,6 +177,8 @@ class DriftSim:
 
     def end_time_step(self) -> None:
         self.algo.end_step(self.t)
+        if self.q_level:
+            self._log_upload_bits()
         cdir = getattr(self.args, "checkpoint_dir", None)
         if cdir:
             ckpt.save(self, os.path.join(cdir, f"step_{self.t:04d}.fdck"))
@@ -220,6 +227,8 @@ class DriftSim:
                 self._small.update(defense=self.defense.defense_type, norm_bound=self.defense.norm_bound, stddev=self.defense.stddev)
             if self.fedprox_mu > 0:
                 self._small["fedprox_mu"] = self.fedprox_mu
+            if self.q_level:
+                self._small.update(compression="qsgd", quantize_level=self.q_level, quantize_bucket=self.q_bucket)
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)
@@ -272,6 +281,18 @@ class DriftSim:
         s = self.spec
         return small_round.fits(s["kind"], s["in"], s["hidden"], s["out"], self.C, self.M, self.t,
                                 server_opt=self.bank.server_opt is not None)
+
+    def upload_bits(self) -> int:
+        """Fixed-length code size in bits of one QSGD upload of this federation (``reference.qsgd_upload_bits``)."""
+        wm = mutils.weight_param_mask(self.bank.spec)[: self.bank.P].bool().cpu()
+        n_train = int(wm.sum())
+        return qsgd_upload_bits(n_train, self.bank.P - n_train, self.q_level, self.q_bucket, wm)
+
+    def _log_upload_bits(self) -> None:
+        """Once per time step: the upload size under QSGD and its ratio to an fp32 upload.  An accounting figure: the
+        engine moves fp32 tensors."""
+        bits = self.upload_bits()
+        self.sink.log({"Comm/UploadBits": bits, "Comm/CompressionRatio": 32.0 * self.bank.P / bits, "iteration": self.t})
 
     def _check_peer_error(self) -> None:
         if self.multi is not None and self.multi["error_np"][0] != 0:

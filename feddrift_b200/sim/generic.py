@@ -11,7 +11,8 @@ architecture and for algorithms that must look at raw client updates before aggr
   gradients land in a flat scratch row, ``ops.adam_amsgrad_rows_`` / ``ops.sgd_rows_`` update the client row;
 * aggregation: ``ops.cluster_aggregate_`` over the ``[C, M, P]`` client arena (K1), with the bank's per-slot server optimizer
   step in its epilogue when one is configured; a robust-aggregation defense first clips (+ noises) the arena rows in place
-  (``ops.robust_clip_slots_``, K10) after the raw-update hooks have seen them;
+  (``ops.robust_clip_slots_``, K10) after the raw-update hooks have seen them; QSGD upload compression quantizes the
+  trained rows in place (``ops.qsgd_slots_``, K17) right after local training, so the hooks see the quantized uploads;
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -31,7 +32,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import ops
-from ..ops.reference import batch_hash, mix32
+from ..ops.reference import batch_hash, compress_seed, mix32
 
 
 def _pair_sampler(st: Dict, c: int, m: int, t: int, nb: torch.Tensor, B: int):
@@ -109,6 +110,8 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
                     cl.params[c, m].copy_(bank.theta[m])
                     _local_steps(sim, c, m, _lazy_client_xy(Xc_all, data, c, T1, S), sampler, seed, rnd, E, use_adam, lr, a.wd, feat_mask)
             cl.n.copy_(torch.from_numpy(n_host), non_blocking=True)
+        if sim.q_level:   # QSGD: each client quantizes its upload against the round-start model before it leaves
+            ops.qsgd_slots_(cl.params, bank.theta, cl.n, sim.q_level, sim.q_bucket, sim.defense_mask, compress_seed(seed, rnd))
         # raw-update hooks (CFL family) may veto the aggregation of this round
         skip = False
         wants_raw = (hasattr(sim.algo, "state") and "cfl" in getattr(sim.algo, "arg", "")) or \
