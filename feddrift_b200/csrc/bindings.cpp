@@ -29,7 +29,7 @@ std::vector<int64_t> fed_round_small(
     std::vector<double> fcfg, std::vector<int64_t> icfg, std::vector<int64_t> peer_inbox,
     c10::optional<Tensor> error_flag, c10::optional<Tensor> counters, std::vector<int64_t> peer_metrics, std::vector<int64_t> host_io,
     c10::optional<Tensor> participation, c10::optional<Tensor> server_s0, c10::optional<Tensor> server_s1,
-    c10::optional<Tensor> server_step) {
+    c10::optional<Tensor> server_step, c10::optional<Tensor> ef_res) {
     CHECK_CUDA_F32(X); CHECK_CUDA_I32(Y); CHECK_CUDA_I32(nsamp); CHECK_CUDA_F32(W); CHECK_CUDA_F32(theta); CHECK_CUDA_I32(opt_step);
     CHECK_CUDA_F32(metrics);
     TORCH_CHECK(X.is_contiguous() && Y.is_contiguous() && nsamp.is_contiguous() && W.is_contiguous() && metrics.is_contiguous(),
@@ -137,6 +137,20 @@ std::vector<int64_t> fed_round_small(
         TORCH_CHECK(s == 0.0 || (b == std::floor(b) && b >= 1.0 && b <= 2147483647.0),
                     "fed_round_small: quantize_bucket must be an integer >= 1");
         p.q_level = (int)s; p.q_bucket = s == 0.0 ? 0 : (int)b;
+    }
+    if (fcfg.size() >= 14) {   // top-k with error feedback: fcfg[13] = entries kept per upload k (0 = off), state ef_res [C, M, P]
+        const double kk = fcfg[13];
+        TORCH_CHECK(kk == std::floor(kk) && kk >= 0.0 && kk <= 2147483647.0, "fed_round_small: topk_k must be an integer >= 0 (0 = off)");
+        p.topk_k = (int)kk;
+        if (p.topk_k > 0) {
+            TORCH_CHECK(p.q_level == 0, "fed_round_small: eftopk and qsgd cannot be combined");
+            TORCH_CHECK(ef_res.has_value() && ef_res->defined(), "fed_round_small: eftopk needs the residual tensor ef_res");
+            const Tensor& er = *ef_res;
+            TORCH_CHECK(er.is_cuda() && er.device() == X.device() && er.scalar_type() == torch::kFloat32 && er.is_contiguous() &&
+                        er.dim() == 3 && er.size(0) == p.C && er.size(1) == p.M && er.size(2) == theta.size(1),
+                        "fed_round_small: ef_res must be a contiguous float32 [C, M, P] tensor on the device of X");
+            p.ef_res = er.data_ptr<float>();
+        }
     }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
@@ -344,6 +358,40 @@ void qsgd_slots(Tensor rows, Tensor theta, c10::optional<Tensor> n, int64_t leve
     CHECK_OK(fdb::qsgd_slots_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)M, np_, mp, (int)R, P,
                                     (int)level, b, reinterpret_cast<unsigned*>(scratch.data_ptr<int>()), (unsigned)seed, cur_stream()),
              "qsgd_slots");
+}
+
+// K18 over an upload arena rows [C, M, P] and its residual [C, M, P] (both contiguous), in place: row (c, m) with
+// n[c, m] > 0 (every row when n is None) keeps its k largest error-corrected entries against its slot's model theta[m, :P]
+// (theta [M, stride >= P], unit column stride) and carries the rest in the residual; entries whose mask byte is 0 pass through.
+void eftopk_slots(Tensor rows, Tensor theta, Tensor residual, c10::optional<Tensor> n, int64_t k, c10::optional<Tensor> mask) {
+    CHECK_CUDA_F32(rows); CHECK_CUDA_F32(theta); CHECK_CUDA_F32(residual);
+    TORCH_CHECK(rows.is_contiguous() && rows.dim() == 3, "eftopk_slots: rows must be a contiguous [C, M, P] tensor");
+    const int64_t M = rows.size(1), P = rows.size(2), R = rows.size(0) * M;
+    TORCH_CHECK(M >= 1 && R <= 65535, "eftopk_slots: need M >= 1 and at most 65535 rows (one grid row each)");
+    TORCH_CHECK(P < (int64_t(1) << 31), "eftopk_slots: rows of 2^31 or more entries are not supported");
+    TORCH_CHECK(residual.device() == rows.device() && residual.is_contiguous() && residual.sizes() == rows.sizes(),
+                "eftopk_slots: residual must be a contiguous float32 tensor of the shape of rows on its device");
+    TORCH_CHECK(theta.device() == rows.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "eftopk_slots: theta must be [M, >= P] with unit column stride on the device of rows");
+    TORCH_CHECK(k >= 1, "eftopk_slots: k must be >= 1");
+    const float* np_ = nullptr;
+    if (n.has_value() && n->defined()) {
+        TORCH_CHECK(n->is_cuda() && n->device() == rows.device() && n->scalar_type() == torch::kFloat32 && n->is_contiguous() &&
+                    n->numel() == R, "eftopk_slots: n must be a contiguous float32 [C, M] tensor on the device of rows");
+        np_ = n->data_ptr<float>();
+    }
+    const unsigned char* mp = nullptr;
+    if (mask.has_value() && mask->defined()) {
+        TORCH_CHECK(mask->is_cuda() && mask->device() == rows.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                    mask->numel() >= P, "eftopk_slots: mask must be a contiguous uint8 [>= P] tensor on the device of rows");
+        mp = mask->data_ptr<unsigned char>();
+    }
+    if (R == 0 || P == 0) return;
+    c10::cuda::CUDAGuard guard(rows.device());
+    auto scratch = torch::empty({fdb::eftopk_scratch_words((int)R, P)}, rows.options().dtype(torch::kInt32));
+    CHECK_OK(fdb::eftopk_slots_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)M, residual.data_ptr<float>(),
+                                      np_, mp, (int)R, P, k, reinterpret_cast<unsigned*>(scratch.data_ptr<int>()), cur_stream()),
+             "eftopk_slots");
 }
 
 // cp: the client arena [C_arena, M, P]; cidx: int32 [C] arena rows of this rank's clients (or None: rows 0..C-1 of cp);
@@ -992,6 +1040,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("robust_clip", &robust_clip);
     m.def("robust_clip_slots", &robust_clip_slots);
     m.def("qsgd_slots", &qsgd_slots);
+    m.def("eftopk_slots", &eftopk_slots);
     m.def("eval_logits", &eval_logits);
     m.def("aue_sqerr", &aue_sqerr);
     m.def("ensemble_vote", &ensemble_vote);

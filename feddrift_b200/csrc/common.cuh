@@ -52,6 +52,10 @@ FDB_DEVICE float qsgd_entry(float x, float th, float sigma, float s, float u) {
     const float q = (u < __fsub_rn(a, l)) ? __fadd_rn(l, 1.f) : l;
     return __fadd_rn(th, copysignf(__fmul_rn(sigma, __fdiv_rn(q, s)), d));
 }
+// top-k with error feedback (ops/reference.py eftopk_slots_): the error-corrected update v = (x − th) + e of one trainable
+// entry, each operation rounded on its own, and its selection key, the bit pattern of |v| (a total order with the index)
+FDB_DEVICE float eftopk_value(float x, float th, float e) { return __fadd_rn(__fsub_rn(x, th), e); }
+FDB_DEVICE unsigned eftopk_key(float v) { return __float_as_uint(v) & 0x7FFFFFFFu; }
 
 // ---------------------------------------------------------------- warp reductions
 FDB_DEVICE float warp_sum(float v) {

@@ -87,10 +87,13 @@ struct BatchSel {
     const int* list; // mode 2: flat sample ids
 };
 
+// upload compression of the publish step (template argument kComp)
+constexpr int kCompNone = 0, kCompQsgd = 1, kCompEfTopk = 2;
+
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
-// its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kQuant: the QSGD variant
-// (p.q_level > 0), separate for the same reason
-template <class Net, bool kDefend, bool kProx, bool kQuant>
+// its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kComp: the upload compression
+// (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0), separate for the same reason
+template <class Net, bool kDefend, bool kProx, int kComp>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P, IN = Net::kIn, OUT = Net::kOut, HID = Net::kHid;
@@ -418,7 +421,7 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     }
                     if (lane == 0) p.opt_step[c * M + m] = ostep;
                 }
-                if constexpr (kQuant) {
+                if constexpr (kComp == kCompQsgd) {
                     // QSGD: the client quantizes its update thl − θ_m (θ_s still holds the round-start models) before the
                     // upload, so client_out, the defense and the average all see the quantized model.  Bucket scales come
                     // from warp_max over the lane-owned columns, one bucket at a time (P is small, so b < P is cheap).
@@ -448,6 +451,51 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                         if (pp < P && sig[q] > 0.f)
                             thl[pp] = qsgd_entry(thl[pp], theta_s[m * P + pp], sig[q], qs,
                                                  uniform_hash(qseed, (uint32_t)k, (unsigned long long)pp));
+                    }
+                }
+                if constexpr (kComp == kCompEfTopk) {
+                    // top-k with error feedback: v = (thl − θ_m) + e over the lane-owned columns (θ_s still holds the
+                    // round-start models), e the pair's residual row.  The rank of column pp is the number of columns j
+                    // with key_j > key_pp, or key_j == key_pp and j < pp, counted over keys broadcast by shuffles (P is
+                    // small); the topk_k columns of rank < topk_k upload thl + e, the others θ and carry v.  Another CTA
+                    // may own this pair in a later round of the launch: the aggregation's cluster barrier orders the
+                    // residual's global writes before those reads, as it does for the optimizer moments.
+                    float* efr = p.ef_res + obase;
+                    float ev[COLS], vv[COLS];
+                    unsigned key[COLS];
+                    int rank[COLS];
+#pragma unroll
+                    for (int q = 0; q < COLS; ++q) {
+                        const int pp = lane + 32 * q;
+                        ev[q] = pp < P ? efr[pp] : 0.f;
+                        vv[q] = pp < P ? eftopk_value(thl[pp], theta_s[m * P + pp], ev[q]) : 0.f;
+                        key[q] = eftopk_key(vv[q]);
+                        rank[q] = 0;
+                    }
+#pragma unroll
+                    for (int q2 = 0; q2 < COLS; ++q2) {
+                        for (int src = 0; src < 32; ++src) {
+                            const unsigned kj = __shfl_sync(0xffffffffu, key[q2], src);
+                            const int j = src + 32 * q2;
+                            if (j < P) {
+#pragma unroll
+                                for (int q = 0; q < COLS; ++q)
+                                    rank[q] += (kj > key[q] || (kj == key[q] && j < lane + 32 * q)) ? 1 : 0;
+                            }
+                        }
+                    }
+#pragma unroll
+                    for (int q = 0; q < COLS; ++q) {
+                        const int pp = lane + 32 * q;
+                        if (pp < P) {
+                            if (rank[q] < p.topk_k) {
+                                if (ev[q] != 0.f) thl[pp] = __fadd_rn(thl[pp], ev[q]);
+                                efr[pp] = 0.f;
+                            } else {
+                                thl[pp] = theta_s[m * P + pp];
+                                efr[pp] = vv[q];
+                            }
+                        }
                     }
                 }
                 const float wgt = ncm_s[k] / tot_s[m];
@@ -760,8 +808,10 @@ __global__ void mlp_eval_matrix_kernel(const float* __restrict__ theta, int thet
 
 // ================================================================================ host launchers
 template <class Net, bool kDefend, bool kProx>
-static auto round_kernel(bool quant) {
-    return quant ? fed_round_small_kernel<Net, kDefend, kProx, true> : fed_round_small_kernel<Net, kDefend, kProx, false>;
+static auto round_kernel(int comp) {
+    return comp == kCompEfTopk ? fed_round_small_kernel<Net, kDefend, kProx, kCompEfTopk>
+         : comp == kCompQsgd   ? fed_round_small_kernel<Net, kDefend, kProx, kCompQsgd>
+                               : fed_round_small_kernel<Net, kDefend, kProx, kCompNone>;
 }
 
 template <class Net>
@@ -780,9 +830,10 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     const SmemLayout L = make_layout<Net>(p.M, p.C, pairs_per_cta, p.sopt_kind != 0);
     const int smem = L.total * (int)sizeof(float);
     if (smem > 227 * 1024) return -2;
-    const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f, quant = p.q_level > 0;
-    auto kern = prox ? (defend ? round_kernel<Net, true, true>(quant) : round_kernel<Net, false, true>(quant))
-                     : (defend ? round_kernel<Net, true, false>(quant) : round_kernel<Net, false, false>(quant));
+    const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f;
+    const int comp = p.topk_k > 0 ? kCompEfTopk : (p.q_level > 0 ? kCompQsgd : kCompNone);
+    auto kern = prox ? (defend ? round_kernel<Net, true, true>(comp) : round_kernel<Net, false, true>(comp))
+                     : (defend ? round_kernel<Net, true, false>(comp) : round_kernel<Net, false, false>(comp));
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return -3;
     cudaLaunchConfig_t cfg{};

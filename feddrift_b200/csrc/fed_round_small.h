@@ -43,6 +43,11 @@ struct RoundParams {
     // bucket q_bucket (common.cuh qsgd_entry, draws uniform_hash(compress_seed(seed, round), c·M + m, e)) before client_out,
     // the defense and the average see it
     int q_level, q_bucket;
+    // top-k with error feedback (topk_k 0 = off): each pair keeps its topk_k largest entries of v = (x − θ_m) + e, e its row
+    // of ef_res [C, M, P] (common.cuh eftopk_value / eftopk_key, ties to the lower index), uploads θ elsewhere and carries
+    // the rest in ef_res, before client_out, the defense and the average see it
+    float* ef_res;
+    int topk_k;
     float* client_out;  // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs

@@ -23,6 +23,12 @@ int robust_clip_launch(float* rows, const float* g, long long g_stride, int M, c
 // n[r] <= 0 are skipped (n may be nullptr), entries with mask 0 pass through; scratch_smax holds R·⌈P / min(b, P)⌉ words
 int qsgd_slots_launch(float* rows, const float* theta, long long t_stride, int M, const float* n, const unsigned char* mask, int R,
                       long long P, int level, long long bucket, unsigned* scratch_smax, unsigned seed, cudaStream_t stream);
+// sparsify.cu (K18): top-k with error feedback of row r of rows [R, P] and its residual row res[r] against
+// theta + (r % M)·t_stride, keeping k trainable entries; rows with n[r] <= 0 are skipped (n may be nullptr), entries with
+// mask 0 pass through; scratch holds eftopk_scratch_words(R, P) words
+long long eftopk_scratch_words(int R, long long P);
+int eftopk_slots_launch(float* rows, const float* theta, long long t_stride, int M, float* res, const float* n,
+                        const unsigned char* mask, int R, long long P, long long k, unsigned* scratch, cudaStream_t stream);
 // aggregate_peer.cu : multi-GPU reduce-scatter + apply + all-gather over NVLink peer memory (cooperative launch)
 int fedavg_reduce_apply_peer_launch(const float* cp, const int* cidx, const float* n, int C, int M, int P, int theta_stride, int world, int rank,
                                     const long long* part_ptrs, const long long* theta_ptrs, const long long* tot_ptrs,

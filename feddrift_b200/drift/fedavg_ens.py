@@ -34,7 +34,7 @@ from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
 from ..core.robustness import make_defense
-from ..ops.reference import compress_seed, compression_params, prox_mu_param
+from ..ops.reference import compress_seed, compression_params, prox_mu_param, topk_k, topk_ratio_param
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
@@ -425,6 +425,17 @@ class _BaseAggregator:
         self._compress_round = 0
         self.models = [self.bank.module(i) for i in range(self.bank.num_models)]
         M, P = self.bank.num_models, self.bank.P
+        # top-k with error feedback (--compression eftopk): each arriving upload is sparsified against bank.theta[m] with the
+        # residual of the CLIENT the worker trained this round (client_sampling's list), not of the worker row; the
+        # aggregator is rebuilt every time step, so the residual starts at zero there
+        self.topk_ratio = topk_ratio_param(getattr(args, "topk_ratio", 0.01))
+        self.topk_k = topk_k(self.topk_ratio, int(wmask.sum())) \
+            if (getattr(args, "compression", "none") or "none") == "eftopk" else 0
+        n_clients = int(getattr(args, "client_num_in_total", worker_num) or worker_num)
+        self.ef_res = torch.zeros(max(n_clients, worker_num), M, P, dtype=torch.float32, device=self.device) \
+            if self.topk_k else None
+        self.bank.ef_res = self.ef_res
+        self._round_clients = None
         self.upload = torch.zeros(worker_num, M, P, dtype=torch.float32, device=self.device)
         self.upload_n = torch.zeros(worker_num, M, dtype=torch.float32, device=self.device)
         self.flag_client_model_uploaded_dict = {i: False for i in range(worker_num)}
@@ -456,6 +467,15 @@ class _BaseAggregator:
                 seed = int(getattr(a, "dummy_arg", 0)) * 7919 + 13 + 1000003 * int(getattr(a, "curr_train_iteration", 0) or 0)
                 ops.qsgd_slots_(self.upload, self.bank.theta, sel.to(self.device), self.q_level, self.q_bucket, self.defense_mask,
                                 compress_seed(seed, self._compress_round))
+        if self.topk_k:   # the client sparsified before it uploaded, with its own residual
+            sel = torch.zeros(1, self.bank.num_models, dtype=torch.float32)
+            for m, (sd, n) in weights_and_num_samples.items():
+                if sd is not None and n > 0:
+                    sel[0, int(m)] = 1.0
+            if bool(sel.any()):
+                c = int(self._round_clients[index]) if self._round_clients is not None else int(index)
+                ops.eftopk_slots_(self.upload[index:index + 1], self.bank.theta, self.ef_res[c:c + 1], sel.to(self.device),
+                                  self.topk_k, self.defense_mask)
         self.flag_client_model_uploaded_dict[index] = True
 
     def check_whether_all_receive(self):
@@ -486,6 +506,13 @@ class _BaseAggregator:
             return list(range(client_num_in_total))
         np.random.seed(round_idx)  # same clients per round across runs (reference behaviour)
         return np.random.choice(range(client_num_in_total), min(client_num_per_round, client_num_in_total), replace=False)
+
+    def sample_round_clients(self, round_idx, client_num_in_total, client_num_per_round):
+        """``client_sampling``, remembered: worker w trains entry w of the list in round ``round_idx``, so the round's
+        uploads find their clients' error-feedback residuals."""
+        idx = self.client_sampling(round_idx, client_num_in_total, client_num_per_round)
+        self._round_clients = idx
+        return idx
 
     def extra_info(self, round_idx):
         return None
@@ -893,7 +920,7 @@ class FedAvgEnsServerManager(ServerManager):
         return 1 + worker % (self.size - 1)
 
     def send_init_msg(self):
-        idx = self.aggregator.client_sampling(self.round_idx, self.args.client_num_in_total, self.args.client_num_per_round)
+        idx = self.aggregator.sample_round_clients(self.round_idx, self.args.client_num_in_total, self.args.client_num_per_round)
         params, extra = self.aggregator.get_global_model_params(), self.aggregator.extra_info(self.round_idx)
         for w in range(self.worker_num):
             self._send(MyMessage.MSG_TYPE_S2C_INIT_CONFIG, self._rank_of(w), params, idx[w], extra, w)
@@ -945,7 +972,7 @@ class FedAvgEnsServerManager(ServerManager):
             self.save_model_params(params)
             self.finish()
             return
-        idx = self.aggregator.client_sampling(self.round_idx, self.args.client_num_in_total, self.args.client_num_per_round)
+        idx = self.aggregator.sample_round_clients(self.round_idx, self.args.client_num_in_total, self.args.client_num_per_round)
         extra = self.aggregator.extra_info(self.round_idx)
         for w in range(self.worker_num):
             self._send(MyMessage.MSG_TYPE_S2C_SYNC_MODEL_TO_CLIENT, self._rank_of(w), params, idx[w], extra, w)

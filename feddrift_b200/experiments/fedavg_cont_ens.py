@@ -58,11 +58,14 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     # the reference's backdoor defense (clipping + Gaussian noise) and carries no (ε, δ) privacy guarantee
     a("--defense_type", type=str, default="none", choices=["none", "norm_diff_clipping", "weak_dp"])
     a("--norm_bound", type=float, default=5.0); a("--stddev", type=float, default=0.025, help="weak_dp noise stddev")
-    # unbiased stochastic quantization (QSGD) of every upload against its round-start cluster model, before the raw-update
-    # hooks, the defense and the average; s levels per sign, one max-norm scale per bucket of b entries
-    a("--compression", type=str, default="none", choices=["none", "qsgd"])
+    # compression of every upload against its round-start cluster model, before the raw-update hooks, the defense and the
+    # average: unbiased stochastic quantization (qsgd; s levels per sign, one max-norm scale per bucket of b entries) or
+    # top-k sparsification with error feedback (eftopk; the ρ·n largest entries of update + residual are sent, the rest is
+    # carried to the client's next upload)
+    a("--compression", type=str, default="none", choices=["none", "qsgd", "eftopk"])
     a("--quantize_level", type=int, default=16, help="QSGD levels s, 1..65535 (s = 1: ternary)")
     a("--quantize_bucket", type=int, default=512, help="QSGD bucket size b (entries per scale), >= 1")
+    a("--topk_ratio", type=float, default=0.01, help="eftopk: fraction ρ of the trainable entries kept, 0 < ρ <= 1")
     # FedProx local training: every client step minimises CE + mu/2‖w − w_m‖², w_m the cluster model it received (0 = off)
     a("--fedprox_mu", type=float, default=0.0)
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)

@@ -18,6 +18,7 @@ Kernel map (SURVEY §2.9 numbering):
   K13 modp_matmul                                 csrc/mpc.cu
   K14 kd_kl_loss   K15 vfl_bce_grad   K16 group_norm   csrc/misc.cu
   K17 qsgd_slots_ (upload quantization)           csrc/compress.cu
+  K18 eftopk_slots_ (top-k + error feedback)      csrc/sparsify.cu
 """
 from __future__ import annotations
 
@@ -102,6 +103,19 @@ def qsgd_slots_(rows, theta, n=None, level: int = 16, bucket: int = 512, weight_
         _ext.load().qsgd_slots(rows, theta, nn, int(level), int(bucket), mask, int(seed) & 0xFFFFFFFF)
         return rows
     return ref.qsgd_slots_(rows, theta, n, level, bucket, weight_mask, seed)
+
+
+def eftopk_slots_(rows, theta, residual, n=None, k: int = 1, weight_mask=None):
+    """K18: top-k with error feedback of an upload arena ``rows [C, M, P]`` and its residual ``residual [C, M, P]``, in
+    place: every row with ``n[c, m] > 0`` keeps its ``k`` largest error-corrected entries against its slot's model
+    ``theta[m, :P]`` (``theta`` may be a padded bank) and carries the rest in the residual.  See
+    ``reference.eftopk_slots_``; returns ``rows``."""
+    if native(rows, theta, residual):
+        mask = weight_mask[: rows.shape[2]].to(torch.uint8).contiguous() if weight_mask is not None else None
+        nn = n.float().contiguous() if n is not None else None
+        _ext.load().eftopk_slots(rows, theta, residual, nn, int(k), mask)
+        return rows
+    return ref.eftopk_slots_(rows, theta, residual, n, k, weight_mask)
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, **kw):

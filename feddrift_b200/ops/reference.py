@@ -216,6 +216,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     goes through ``qsgd_slots_`` against the round-start θ with seed ``compress_seed(seed, rnd)`` (the client quantizes
     before it uploads), so ``client_out``, the defense and the average see the quantized model.  ``client_out [C, M, P]``:
     the local models as uploaded (quantized, undefended) of the pairs that trained in the last round are written there.
+    ``compression`` 'eftopk' with ``topk_ratio`` ρ (0.01) and state ``ef_residual [C, M, P]`` (created zero when missing,
+    updated in place like the optimizer moments): at the same point every trained pair's local model goes through
+    ``eftopk_slots_`` against the round-start θ with k = ``topk_k(ρ, P)``; ``client_out``, the defense and the average see
+    the sparsified model.
     ``fedprox_mu`` (absent or 0: off): every local
     step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
     (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
@@ -246,6 +250,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     prox_mu = prox_mu_param(st.get("fedprox_mu", 0.0))
     q_level, q_bucket = compression_params(st.get("compression") or "none", st.get("quantize_level", 16),
                                            st.get("quantize_bucket", 512))
+    ef_ratio = topk_ratio_param(st.get("topk_ratio", 0.01))
+    ef_k = topk_k(ef_ratio, P) if (st.get("compression") or "none") == "eftopk" else 0
+    if ef_k and st.get("ef_residual") is None:
+        st["ef_residual"] = torch.zeros(C, M, P, dtype=torch.float32)
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -293,6 +301,13 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
             for (c, m), (p, _) in locals_.items():
                 up[c, m], trained[c, m] = p, 1.0
             qsgd_slots_(up, theta, trained, q_level, q_bucket, None, compress_seed(seed, rnd))
+            locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
+        if ef_k and locals_:   # top-k with error feedback: each client sparsifies its upload against the round-start θ_m
+            up = torch.zeros(C, M, P, dtype=torch.float32)
+            trained = torch.zeros(C, M)
+            for (c, m), (p, _) in locals_.items():
+                up[c, m], trained[c, m] = p, 1.0
+            eftopk_slots_(up, theta, st["ef_residual"], trained, ef_k, None)
             locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
         if client_out is not None and r == rounds - 1:
             for (c, m), (p, _) in locals_.items():
@@ -483,7 +498,7 @@ def robust_clip_slots_(rows: torch.Tensor, theta: torch.Tensor, n=None, bound: f
     return norms
 
 
-COMPRESSIONS = ("none", "qsgd")
+COMPRESSIONS = ("none", "qsgd", "eftopk")
 
 
 def _int_param(name: str, v) -> int:
@@ -500,7 +515,7 @@ def _int_param(name: str, v) -> int:
 
 def compression_params(compression: str, quantize_level, quantize_bucket) -> Tuple[int, int]:
     """Validated ``(level s, bucket b)`` of the upload compression (``--compression`` / ``--quantize_level`` /
-    ``--quantize_bucket``); ``(0, 0)`` for ``none``.  Raises ``ValueError`` for an unknown compression, a level that is not
+    ``--quantize_bucket``); ``(0, 0)`` for ``none`` and ``eftopk`` (QSGD off).  Raises ``ValueError`` for an unknown compression, a level that is not
     an integer in [1, 65535], or a bucket that is not an integer ≥ 1 (whatever the compression)."""
     if compression not in COMPRESSIONS:
         raise ValueError(f"compression must be one of {', '.join(COMPRESSIONS)} (got {compression!r})")
@@ -589,6 +604,80 @@ def qsgd_upload_bits(P_train: int, P_other: int, level: int, bucket: int, weight
     else:
         buckets = (P_train + b - 1) // b
     return 32 * buckets + (1 + int(s).bit_length()) * P_train + 32 * P_other
+
+
+def topk_ratio_param(rho) -> float:
+    """Validated ``--topk_ratio`` ρ (fraction of the trainable entries an ``eftopk`` upload keeps): a finite number with
+    0 < ρ ≤ 1, checked whatever the compression.  Raises ``ValueError`` otherwise."""
+    if isinstance(rho, bool):
+        raise ValueError(f"topk_ratio must be a number in (0, 1] (got {rho!r})")
+    try:
+        f = float(rho)
+    except (TypeError, ValueError):
+        raise ValueError(f"topk_ratio must be a number in (0, 1] (got {rho!r})") from None
+    if not (math.isfinite(f) and 0.0 < f <= 1.0):
+        raise ValueError(f"topk_ratio must be a number in (0, 1] (got {rho!r})")
+    return f
+
+
+def topk_k(rho, n_train: int) -> int:
+    """Entries kept per ``eftopk`` upload: max(1, min(n_train, ⌊ρ·n_train + 0.5⌋)) over ``n_train`` trainable entries
+    (round half up in float64; ⌈ρ·n⌉ would give 4 for ρ = 0.1, n = 30)."""
+    f = topk_ratio_param(rho)
+    n_train = int(n_train)
+    return max(1, min(n_train, int(math.floor(f * n_train + 0.5))))
+
+
+def eftopk_slots_(rows: torch.Tensor, theta: torch.Tensor, residual: torch.Tensor, n=None, k: int = 1,
+                  weight_mask=None) -> torch.Tensor:
+    """Top-k sparsification with error feedback (K18) over an upload arena ``rows [C, M, P]`` and its residual
+    ``residual [C, M, P]``, both in place.  Row (c, m) with ``n[c, m] > 0`` (every row when ``n`` is None), with
+    θ_m = ``theta[m, :P]``, x the row and e its residual:
+
+    * v = (x − θ_m) + e over the trainable entries (``weight_mask`` True), each operation rounded in fp32;
+    * key = bit pattern of |v| as uint32; the k entries with the largest keys are selected, ties going to the lower flat
+      index (a total order, so GPU and CPU agree bit for bit);
+    * a selected entry uploads x + e (x itself when e == 0) and its residual becomes 0;
+    * an unselected trainable entry uploads θ_e and its residual becomes v;
+    * non-trainable entries pass through and keep their residual.
+
+    Rows with n ≤ 0 keep both their upload and their residual.  With k ≥ the trainable count every entry is selected, so
+    a zero residual stays zero and the uploads are unchanged.  Returns ``rows``."""
+    C, M, P = rows.shape
+    k = int(k)
+    if k < 1:
+        raise ValueError(f"eftopk: k must be >= 1 (got {k})")
+    if tuple(residual.shape) != (C, M, P):
+        raise ValueError("eftopk: residual must have the shape of rows")
+    if C * M == 0 or P == 0:
+        return rows
+    th = theta[:, :P].to(rows.device)
+    sel = torch.ones(C, M, dtype=torch.bool) if n is None else (n.detach().cpu().reshape(C, M) > 0)
+    wm = torch.ones(P, dtype=torch.bool, device=rows.device) if weight_mask is None else \
+        weight_mask[:P].to(rows.device).bool()
+    cand = wm.nonzero().flatten()
+    kk = min(k, int(cand.numel()))
+    for c, m in sel.nonzero().tolist():
+        x, e = rows[c, m], residual[c, m]
+        v = (x - th[m]) + e
+        key = v.view(torch.int32).to(torch.int64) & 0x7FFFFFFF
+        order = torch.sort(key[cand], descending=True, stable=True).indices[:kk]
+        chosen = torch.zeros(P, dtype=torch.bool, device=rows.device)
+        chosen[cand[order]] = True
+        up = torch.where(e == 0, x, x + e)
+        new_x = torch.where(chosen, up, torch.where(wm, th[m], x))
+        new_e = torch.where(chosen, torch.zeros_like(e), torch.where(wm, v, e))
+        x.copy_(new_x)
+        e.copy_(new_e)
+    return rows
+
+
+def topk_upload_bits(P_train: int, P_other: int, k: int) -> int:
+    """Size in bits of one ``eftopk`` upload: a 32-bit value and a ⌈log₂ P⌉-bit index (bit_length(P − 1)) per kept entry,
+    plus 32 bits per non-trainable entry (sent raw), with P = P_train + P_other."""
+    P_train, P_other, k = int(P_train), int(P_other), int(k)
+    P = P_train + P_other
+    return k * (32 + max(P - 1, 0).bit_length()) + 32 * P_other
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

@@ -141,11 +141,23 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer / defense slots, unread when off
         fcfg.append(prox_mu)
     compression = st.get("compression") or "none"
-    if compression != "none":   # QSGD in the publish step (reference.fed_round_small documents the keys)
+    ef_res = None
+    if compression == "qsgd":   # QSGD in the publish step (reference.fed_round_small documents the keys)
         from .reference import compression_params
         q = compression_params(compression, st.get("quantize_level", 16), st.get("quantize_bucket", 512))
         fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer / defense / FedProx slots, unread when off
         fcfg += [float(q[0]), float(q[1])]
+    elif compression == "eftopk":   # top-k with error feedback in the publish step; QSGD's slots stay (0, 0)
+        from .reference import topk_k
+        k = topk_k(st.get("topk_ratio", 0.01), theta.shape[1])
+        ef_res = st.get("ef_residual")
+        if ef_res is None:
+            ef_res = st["ef_residual"] = torch.zeros(C, M, theta.shape[1], dtype=torch.float32, device=dev)
+        fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer / defense / FedProx / QSGD slots
+        fcfg.append(float(k))
+    elif compression != "none":
+        from .reference import compression_params
+        compression_params(compression, 16, 512)   # raises for an unknown compression
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out
@@ -159,7 +171,7 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         list(mg["inbox_ptrs"]) if mg else [], mg.get("error_flag") if mg else None,
         st.get("counters"), peer_metrics, [int(v) for v in st["host_io"]] if st.get("host_io") else [],
         cache["participation"], st.get("server_s0") if sopt else None, st.get("server_s1") if sopt else None,
-        st.get("server_step") if sopt else None)
+        st.get("server_step") if sopt else None, ef_res)
     if mg:
         mg["flag_base"] = int(mg["flag_base"]) + rounds
     if st.get("counters") is not None:

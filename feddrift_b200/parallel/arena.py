@@ -67,6 +67,9 @@ class ModelBank:
         # per-slot server optimizer state (ops.server_opt.SlotServerOpt) or None: a slot that is re-initialised or
         # overwritten starts its optimizer afresh, so reinit / copy reset the destination slot's state here
         self.server_opt = None
+        # the clients' error-feedback residual [C, M, P] of --compression eftopk or None: residual built up against a slot's
+        # old model means nothing for its new one, so reinit / copy zero the destination slot's column for every client
+        self.ef_res = None
         self.float_mask = torch.zeros(self.P, dtype=torch.bool)
         for _, _, dt, off, n in self.spec:
             self.float_mask[off:off + n] = bool(dt.is_floating_point)
@@ -98,11 +101,15 @@ class ModelBank:
             self.theta[dst].copy_(self.theta[src])
             if self.server_opt is not None:
                 self.server_opt.reset(dst)
+            if self.ef_res is not None:
+                self.ef_res[:, dst].zero_()
 
     def reinit(self, m: int) -> None:
         self.theta[m].copy_(self.init_row)
         if self.server_opt is not None:
             self.server_opt.reset(m)
+        if self.ef_res is not None:
+            self.ef_res[:, m].zero_()
 
     def reset_parameters_random(self, m: int, generator: Optional[torch.Generator] = None) -> None:
         """Fresh (NOT reseeded) init — the IFCA 'hard' path at t=0 calls ``reset_parameters`` directly
@@ -172,7 +179,7 @@ class ClientArena:
     inside a time step and is reset between time steps (the reference gets this implicitly from
     relaunching the process per time step — ``FedAvgEnsTrainer.py:25-33``, SURVEY §7.3)."""
 
-    def __init__(self, num_clients: int, num_models: int, P: int, device="cpu", adam: bool = True):
+    def __init__(self, num_clients: int, num_models: int, P: int, device="cpu", adam: bool = True, ef: bool = False):
         self.C, self.M, self.P = num_clients, num_models, P
         self.device = torch.device(device)
         z = lambda: torch.zeros(num_clients, num_models, P, dtype=torch.float32, device=self.device)  # noqa: E731
@@ -182,9 +189,12 @@ class ClientArena:
         self.vmax = z() if adam else None
         self.step = torch.zeros(num_clients, num_models, dtype=torch.int32, device=self.device)
         self.n = torch.zeros(num_clients, num_models, dtype=torch.float32, device=self.device)
+        # error-feedback residual of --compression eftopk (the part of each (client, slot) update not uploaded yet)
+        self.ef_res = z() if ef else None
 
     def reset_optimizer(self) -> None:
-        for t in (self.m, self.v, self.vmax):
+        """Start of a time step: the client optimizer state and the error-feedback residual start from zero."""
+        for t in (self.m, self.v, self.vmax, self.ef_res):
             if t is not None:
                 t.zero_()
         self.step.zero_()

@@ -36,7 +36,8 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import compression_params, prox_mu_param, qsgd_upload_bits
+from ..ops.reference import (compression_params, prox_mu_param, qsgd_upload_bits, topk_k, topk_ratio_param,
+                             topk_upload_bits)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -52,7 +53,7 @@ DEFAULTS = dict(
     is_mobile=0, gpu_num_per_server=1, data_dir=None, checkpoint_dir=None, rounds_per_launch=0,
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
-    compression="none", quantize_level=16, quantize_bucket=512,
+    compression="none", quantize_level=16, quantize_bucket=512, topk_ratio=0.01,
 )
 
 
@@ -106,6 +107,11 @@ class DriftSim:
         # training; (q_level, q_bucket) = (0, 0) is off
         self.q_level, self.q_bucket = compression_params(getattr(args, "compression", "none") or "none",
                                                          getattr(args, "quantize_level", 16), getattr(args, "quantize_bucket", 512))
+        # top-k with error feedback (--compression eftopk): every upload keeps its topk_k largest error-corrected trainable
+        # entries; the rest is carried in the clients' residual (ClientArena.ef_res).  topk_k 0 is off
+        self.topk_ratio = topk_ratio_param(getattr(args, "topk_ratio", 0.01))
+        n_train = int(wmask[: self.bank.P].sum())
+        self.topk_k = topk_k(self.topk_ratio, n_train) if (getattr(args, "compression", "none") or "none") == "eftopk" else 0
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -118,7 +124,8 @@ class DriftSim:
         self.multi = None
         self.shard_clients = False   # generic path: shard clients over torch.distributed ranks + PeerAggregator
         self.clients = ClientArena(self.C, self.M, self.bank.P, self.device,
-                                   adam=(args.client_optimizer != "sgd"))
+                                   adam=(args.client_optimizer != "sgd"), ef=self.topk_k > 0)
+        self.bank.ef_res = self.clients.ef_res
         self.timings = {"cluster_s": 0.0, "rounds_s": 0.0}
 
     def _participation_table(self) -> Optional[np.ndarray]:
@@ -177,7 +184,7 @@ class DriftSim:
 
     def end_time_step(self) -> None:
         self.algo.end_step(self.t)
-        if self.q_level:
+        if self.q_level or self.topk_k:
             self._log_upload_bits()
         cdir = getattr(self.args, "checkpoint_dir", None)
         if cdir:
@@ -229,6 +236,8 @@ class DriftSim:
                 self._small["fedprox_mu"] = self.fedprox_mu
             if self.q_level:
                 self._small.update(compression="qsgd", quantize_level=self.q_level, quantize_bucket=self.q_bucket)
+            if self.topk_k:   # the arena's residual: the kernel reads and writes it in place
+                self._small.update(compression="eftopk", topk_ratio=self.topk_ratio, ef_residual=self.clients.ef_res)
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)
@@ -283,14 +292,17 @@ class DriftSim:
                                 server_opt=self.bank.server_opt is not None)
 
     def upload_bits(self) -> int:
-        """Fixed-length code size in bits of one QSGD upload of this federation (``reference.qsgd_upload_bits``)."""
+        """Size in bits of one compressed upload of this federation (``reference.qsgd_upload_bits`` under QSGD,
+        ``reference.topk_upload_bits`` under eftopk)."""
         wm = mutils.weight_param_mask(self.bank.spec)[: self.bank.P].bool().cpu()
         n_train = int(wm.sum())
+        if self.topk_k:
+            return topk_upload_bits(n_train, self.bank.P - n_train, self.topk_k)
         return qsgd_upload_bits(n_train, self.bank.P - n_train, self.q_level, self.q_bucket, wm)
 
     def _log_upload_bits(self) -> None:
-        """Once per time step: the upload size under QSGD and its ratio to an fp32 upload.  An accounting figure: the
-        engine moves fp32 tensors."""
+        """Once per time step: the upload size under QSGD or eftopk and its ratio to an fp32 upload.  An accounting
+        figure: the engine moves fp32 tensors."""
         bits = self.upload_bits()
         self.sink.log({"Comm/UploadBits": bits, "Comm/CompressionRatio": 32.0 * self.bank.P / bits, "iteration": self.t})
 
@@ -363,7 +375,8 @@ class DriftSim:
         # cross-GPU epoch stays advanced because the peers have seen it)
         cl = self.clients
         so = self.bank.server_opt
-        snap = [(x, x.clone()) for x in (self.bank.theta, cl.m, cl.v, cl.vmax, cl.step, st.get("W"), *(so.tensors() if so else ()))
+        snap = [(x, x.clone()) for x in (self.bank.theta, cl.m, cl.v, cl.vmax, cl.step, cl.ef_res, st.get("W"),
+                                         *(so.tensors() if so else ()))
                 if isinstance(x, torch.Tensor)]
         cnt = st.get("counters")
         cnt0 = cnt[0:1].clone() if isinstance(cnt, torch.Tensor) else None

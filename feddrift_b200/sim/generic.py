@@ -13,6 +13,7 @@ architecture and for algorithms that must look at raw client updates before aggr
   step in its epilogue when one is configured; a robust-aggregation defense first clips (+ noises) the arena rows in place
   (``ops.robust_clip_slots_``, K10) after the raw-update hooks have seen them; QSGD upload compression quantizes the
   trained rows in place (``ops.qsgd_slots_``, K17) right after local training, so the hooks see the quantized uploads;
+  top-k with error feedback sparsifies them there instead (``ops.eftopk_slots_``, K18, residual ``ClientArena.ef_res``);
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -112,6 +113,8 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
             cl.n.copy_(torch.from_numpy(n_host), non_blocking=True)
         if sim.q_level:   # QSGD: each client quantizes its upload against the round-start model before it leaves
             ops.qsgd_slots_(cl.params, bank.theta, cl.n, sim.q_level, sim.q_bucket, sim.defense_mask, compress_seed(seed, rnd))
+        if sim.topk_k:   # top-k with error feedback: each client sparsifies its upload and keeps the rest in its residual
+            ops.eftopk_slots_(cl.params, bank.theta, cl.ef_res, cl.n, sim.topk_k, sim.defense_mask)
         # raw-update hooks (CFL family) may veto the aggregation of this round
         skip = False
         wants_raw = (hasattr(sim.algo, "state") and "cfl" in getattr(sim.algo, "arg", "")) or \
