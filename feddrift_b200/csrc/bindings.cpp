@@ -152,6 +152,17 @@ std::vector<int64_t> fed_round_small(
             p.ef_res = er.data_ptr<float>();
         }
     }
+    if (fcfg.size() >= 16) {   // aggregation rule: fcfg[14] = 0 mean / 1 median / 2 trimmed mean, fcfg[15] = trim ratio
+        const double rule = fcfg[14], beta = fcfg[15];
+        TORCH_CHECK(rule == 0.0 || rule == 1.0 || rule == 2.0, "fed_round_small: aggregation rule must be 0 (mean), 1 (median) or 2 (trimmed_mean)");
+        TORCH_CHECK(std::isfinite(beta) && beta >= 0.0 && beta < 0.5, "fed_round_small: trim_ratio must be in [0, 0.5)");
+        p.agg_rule = (int)rule; p.trim_ratio = (float)beta;
+        if (p.agg_rule != 0) {
+            TORCH_CHECK(p.world == 1, "fed_round_small: a robust aggregation rule is single-GPU only");
+            TORCH_CHECK(2 * (int64_t)p.C <= 33 * theta.size(1),
+                        "fed_round_small: too many clients for the robust aggregation scratch (use fed_round_small_fits to route)");
+        }
+    }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
     TORCH_CHECK(rc != -1, "fed_round_small: MLP shape (", kind, ",", din, ",", hid, ",", dout, ") is not instantiated");
@@ -160,8 +171,9 @@ std::vector<int64_t> fed_round_small(
     return {info.cluster, info.threads, info.smem_bytes};
 }
 
-bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur, bool server_opt) {
-    return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt) != 0;
+bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur, bool server_opt,
+                          bool robust) {
+    return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt, robust) != 0;
 }
 
 bool fed_round_small_supported(int64_t kind, int64_t din, int64_t hid, int64_t dout) {
@@ -392,6 +404,62 @@ void eftopk_slots(Tensor rows, Tensor theta, Tensor residual, c10::optional<Tens
     CHECK_OK(fdb::eftopk_slots_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)M, residual.data_ptr<float>(),
                                       np_, mp, (int)R, P, k, reinterpret_cast<unsigned*>(scratch.data_ptr<int>()), cur_stream()),
              "eftopk_slots");
+}
+
+// K19: coordinate-wise median (rule 1) or trimmed mean (rule 2, trim ratio beta) of the participants (n[c, m] > 0) of every
+// slot of an upload arena cp [C, M, P] (contiguous) into theta [M, stride >= P] (unit column stride).  opt_kind 1..4 runs the
+// per-slot server optimizer on theta_m - statistic (state [M, P], counters steps [M] advanced for every slot with a
+// participant, mask [P] uint8 keeps entries with mask 0 at the statistic), as cluster_aggregate_slots does for the mean.
+// Returns the participant counts [M] (float32).
+Tensor robust_aggregate_slots(Tensor theta, Tensor cp, Tensor n, int64_t rule, double beta, int64_t opt_kind, double lr, double momentum,
+                              double eps, c10::optional<Tensor> s0, c10::optional<Tensor> s1, c10::optional<Tensor> steps,
+                              c10::optional<Tensor> mask) {
+    CHECK_CUDA_F32(theta); CHECK_CUDA_F32(cp); CHECK_CUDA_F32(n);
+    TORCH_CHECK(rule == 1 || rule == 2, "robust_aggregate_slots: rule must be 1 (median) or 2 (trimmed_mean)");
+    TORCH_CHECK(std::isfinite(beta) && beta >= 0.0 && beta < 0.5, "robust_aggregate_slots: trim ratio must be in [0, 0.5)");
+    TORCH_CHECK(cp.is_contiguous() && cp.dim() == 3, "robust_aggregate_slots: cp must be a contiguous [C, M, P] tensor");
+    const int64_t C = cp.size(0), M = cp.size(1), P = cp.size(2);
+    TORCH_CHECK(C < (int64_t(1) << 31) && M <= 65535, "robust_aggregate_slots: need C < 2^31 and M <= 65535");
+    TORCH_CHECK(n.device() == cp.device() && n.is_contiguous() && n.numel() == C * M,
+                "robust_aggregate_slots: n must be a contiguous float32 [C, M] tensor on the device of cp");
+    TORCH_CHECK(theta.device() == cp.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "robust_aggregate_slots: theta must be [M, >= P] with unit column stride on the device of cp");
+    float *p0 = nullptr, *p1 = nullptr;
+    int* sp = nullptr;
+    const unsigned char* mp = nullptr;
+    if (opt_kind != 0) {
+        TORCH_CHECK(opt_kind >= 1 && opt_kind <= 4, "robust_aggregate_slots: server optimizer kind must be 0..4");
+        for (const auto* t : {&s0, &s1}) {
+            if (t->has_value() && (*t)->defined()) {
+                CHECK_CUDA_F32(**t);
+                TORCH_CHECK((*t)->is_contiguous() && (*t)->dim() == 2 && (*t)->size(0) == M && (*t)->size(1) == P &&
+                            (*t)->device() == cp.device(),
+                            "robust_aggregate_slots: optimizer state must be contiguous [M, P] on the device of cp");
+            }
+        }
+        p0 = opt_ptr<float>(s0); p1 = opt_ptr<float>(s1);
+        TORCH_CHECK(p0 || (opt_kind == 1 && momentum == 0.0), "robust_aggregate_slots: this optimizer needs s0");
+        TORCH_CHECK(p1 || opt_kind == 1 || opt_kind == 3, "robust_aggregate_slots: this optimizer needs s1");
+        TORCH_CHECK(steps.has_value() && steps->defined(), "robust_aggregate_slots: a server optimizer needs the step counters");
+        CHECK_CUDA_I32(*steps);
+        TORCH_CHECK(steps->is_contiguous() && steps->numel() == M && steps->device() == cp.device(),
+                    "robust_aggregate_slots: steps must be a contiguous int32 [M] tensor on the device of cp");
+        sp = steps->data_ptr<int>();
+        if (mask.has_value() && mask->defined()) {
+            TORCH_CHECK(mask->is_cuda() && mask->device() == cp.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                        mask->numel() == P, "robust_aggregate_slots: mask must be a contiguous uint8 [P] tensor on the device of cp");
+            mp = mask->data_ptr<unsigned char>();
+        }
+    }
+    c10::cuda::CUDAGuard guard(cp.device());
+    auto counts = (n.view({C, M}) > 0).sum(0).to(torch::kFloat32);
+    const int rc = fdb::robust_aggregate_launch(theta.data_ptr<float>(), theta.stride(0), cp.data_ptr<float>(), n.data_ptr<float>(), (int)C,
+                                                (int)M, P, rule == 1 ? 1 : 0, (float)beta, (int)opt_kind, (float)lr, (float)momentum,
+                                                0.9f, 0.999f, (float)eps, p0, p1, sp, mp, cur_stream());
+    TORCH_CHECK(rc != -2, "robust_aggregate_slots: too many clients for the shared-memory staging of one column tile");
+    TORCH_CHECK(rc == 0, "robust_aggregate_slots: kernel launch failed");
+    if (sp) steps->add_((counts > 0).to(torch::kInt32));   // after the launch (same stream), as cluster_aggregate_slots does
+    return counts;
 }
 
 // cp: the client arena [C_arena, M, P]; cidx: int32 [C] arena rows of this rank's clients (or None: rows 0..C-1 of cp);
@@ -1041,6 +1109,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("robust_clip_slots", &robust_clip_slots);
     m.def("qsgd_slots", &qsgd_slots);
     m.def("eftopk_slots", &eftopk_slots);
+    m.def("robust_aggregate_slots", &robust_aggregate_slots);
     m.def("eval_logits", &eval_logits);
     m.def("aue_sqerr", &aue_sqerr);
     m.def("ensemble_vote", &ensemble_vote);

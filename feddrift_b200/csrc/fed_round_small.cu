@@ -80,6 +80,62 @@ FDB_DEVICE void group_barrier(int wpp, int gidx) {
     else asm volatile("bar.sync %0, %1;" ::"r"(1 + gidx), "r"(wpp * 32) : "memory");
 }
 
+// Robust aggregation phase (RoundParams::agg_rule != 0): the median / trimmed mean of ops/reference.py
+// robust_aggregate_slots_ for the columns e ≡ crank (mod G) of the [M, P] models, written into part[e] (θ_s[e] for a slot
+// without participants).  One warp per column: the slot's uploads are gathered over DSMEM into scratch[0, n) in pair order,
+// lane i ranks its values against the column and scatters them to scratch[n + rank]; lane 0 sums the kept ranks in order and
+// divides once.  scratch holds 2n floats (fed_round_small_fits checks 2·C ≤ 33·P, the size of a warp's gbuf).
+template <int P>
+FDB_DEVICE void robust_columns(float* slot_s, const int* pairs_s, int npairs, const float* tot_s, const float* theta_s, float* part,
+                               float* scratch, int M, int G, int crank, int warp, int NW, int lane, bool median, float beta) {
+    cg::cluster_group cluster = cg::this_cluster();
+    const int MP = M * P;
+    const unsigned lt = (1u << lane) - 1u;
+    for (int e = crank + G * warp; e < MP; e += G * NW) {
+        const int m = e / P, pp = e - m * P;
+        if (!(tot_s[m] > 0.f)) continue;
+        int n = 0;
+        bool nan = false;
+        for (int i0 = 0; i0 < npairs; i0 += 32) {
+            const int i = i0 + lane;
+            const bool on = i < npairs && pairs_s[i] % M == m;
+            const unsigned bal = __ballot_sync(0xffffffffu, on);
+            if (on) {
+                const float v = *(cluster.map_shared_rank(slot_s + (i / G) * P + pp, i % G));
+                nan |= isnan(v);
+                scratch[n + __popc(bal & lt)] = v;
+            }
+            n += __popc(bal);
+        }
+        nan = __any_sync(0xffffffffu, nan);
+        __syncwarp();
+        if (!nan)
+            for (int i = lane; i < n; i += 32) {
+                const float a = scratch[i];
+                int rk = 0;
+                for (int j = 0; j < n; ++j) {
+                    const float x = scratch[j];
+                    rk += (x < a || (x == a && j < i)) ? 1 : 0;
+                }
+                scratch[n + rk] = a;
+            }
+        __syncwarp();
+        if (lane == 0) {
+            float v = theta_s[e];
+            if (nan) {
+                v = __int_as_float(0x7FC00000);
+            } else if (n > 0) {
+                const int b = median ? (n - 1) / 2 : (int)floorf(__fmul_rn(beta, (float)n));
+                float s = scratch[n + b];
+                for (int j = b + 1; j < n - b; ++j) s = __fadd_rn(s, scratch[n + j]);
+                v = __fdiv_rn(s, (float)(n - 2 * b));
+            }
+            part[e] = v;
+        }
+        __syncwarp();
+    }
+}
+
 // sample coordinates of element i of the current mini-batch
 struct BatchSel {
     int mode;        // 0/1: contiguous [lo, lo+n) of (tb, c);  2: list
@@ -92,8 +148,9 @@ constexpr int kCompNone = 0, kCompQsgd = 1, kCompEfTopk = 2;
 
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
 // its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kComp: the upload compression
-// (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0), separate for the same reason
-template <class Net, bool kDefend, bool kProx, int kComp>
+// (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0) and kRobust: a median / trimmed-mean aggregation rule
+// (p.agg_rule != 0), separate for the same reason
+template <class Net, bool kDefend, bool kProx, int kComp, bool kRobust>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P, IN = Net::kIn, OUT = Net::kOut, HID = Net::kHid;
@@ -498,7 +555,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                         }
                     }
                 }
-                const float wgt = ncm_s[k] / tot_s[m];
+                // a robust rule ranks the uploads themselves: slot_s holds them unweighted (x · 1 == x)
+                const float wgt = kRobust ? 1.f : ncm_s[k] / tot_s[m];
                 float dscale = 1.f;
                 bool defend = false;
                 if constexpr (kDefend) {
@@ -539,13 +597,22 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
 
         // ------------------------------------------------------------------ aggregation
         if (!p.skip_aggregate) {
-            const int n_local = (npairs > crank) ? (npairs - crank + G - 1) / G : 0;
-            for (int e = tid; e < MP; e += blockDim.x) {
-                const int m = e / P, pp = e - m * P;
-                float acc = 0.f;
-                for (int li = 0; li < n_local; ++li)
-                    if (slot_model[li] == m) acc += slot_s[li * P + pp];
-                part_s[buf * MP + e] = acc;
+            if constexpr (!kRobust) {
+                const int n_local = (npairs > crank) ? (npairs - crank + G - 1) / G : 0;
+                for (int e = tid; e < MP; e += blockDim.x) {
+                    const int m = e / P, pp = e - m * P;
+                    float acc = 0.f;
+                    for (int li = 0; li < n_local; ++li)
+                        if (slot_model[li] == m) acc += slot_s[li * P + pp];
+                    part_s[buf * MP + e] = acc;
+                }
+            } else {
+                // robust rule: every CTA's published uploads become visible, then CTA crank computes the statistic of the
+                // columns e ≡ crank (mod G) into its part_s, one warp per column over DSMEM (pair i of the compacted list
+                // lives in CTA i mod G, slot i / G; pairs_s is the same in every CTA), with the warp's gbuf as scratch
+                if (G > 1) cluster.sync(); else __syncthreads();
+                robust_columns<P>(slot_s, pairs_s, npairs, tot_s, theta_s, part_s + buf * MP, smem + L.gbuf + warp * (P * 33),
+                                  M, G, crank, warp, NW, lane, p.agg_rule == 1, p.trim_ratio);
             }
             if (G > 1) cluster.sync(); else __syncthreads();
             if (p.world == 1) {
@@ -553,7 +620,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     const int m = e / P;
                     if (tot_s[m] > 0.f) {
                         float v = 0.f;
-                        for (int rk = 0; rk < G; ++rk) v += *(cluster.map_shared_rank(part_s + buf * MP + e, rk));
+                        if constexpr (kRobust) v = *(cluster.map_shared_rank(part_s + buf * MP + e, e % G));   // the column's owner
+                        else for (int rk = 0; rk < G; ++rk) v += *(cluster.map_shared_rank(part_s + buf * MP + e, rk));
                         if (p.sopt_kind) {
                             const float ts = (float)(sstep_s[m] + 1);
                             v = server_opt_update(p.sopt_kind, theta_s[e], v, sopt_s, sopt_s + MP, (size_t)e, p.sopt_lr,
@@ -807,11 +875,16 @@ __global__ void mlp_eval_matrix_kernel(const float* __restrict__ theta, int thet
 }
 
 // ================================================================================ host launchers
+template <class Net, bool kDefend, bool kProx, bool kRobust>
+static auto round_kernel_c(int comp) {
+    return comp == kCompEfTopk ? fed_round_small_kernel<Net, kDefend, kProx, kCompEfTopk, kRobust>
+         : comp == kCompQsgd   ? fed_round_small_kernel<Net, kDefend, kProx, kCompQsgd, kRobust>
+                               : fed_round_small_kernel<Net, kDefend, kProx, kCompNone, kRobust>;
+}
+
 template <class Net, bool kDefend, bool kProx>
-static auto round_kernel(int comp) {
-    return comp == kCompEfTopk ? fed_round_small_kernel<Net, kDefend, kProx, kCompEfTopk>
-         : comp == kCompQsgd   ? fed_round_small_kernel<Net, kDefend, kProx, kCompQsgd>
-                               : fed_round_small_kernel<Net, kDefend, kProx, kCompNone>;
+static auto round_kernel(int comp, bool robust) {
+    return robust ? round_kernel_c<Net, kDefend, kProx, true>(comp) : round_kernel_c<Net, kDefend, kProx, false>(comp);
 }
 
 template <class Net>
@@ -832,8 +905,9 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     if (smem > 227 * 1024) return -2;
     const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f;
     const int comp = p.topk_k > 0 ? kCompEfTopk : (p.q_level > 0 ? kCompQsgd : kCompNone);
-    auto kern = prox ? (defend ? round_kernel<Net, true, true>(comp) : round_kernel<Net, false, true>(comp))
-                     : (defend ? round_kernel<Net, true, false>(comp) : round_kernel<Net, false, false>(comp));
+    const bool robust = p.agg_rule != 0;
+    auto kern = prox ? (defend ? round_kernel<Net, true, true>(comp, robust) : round_kernel<Net, false, true>(comp, robust))
+                     : (defend ? round_kernel<Net, true, false>(comp, robust) : round_kernel<Net, false, false>(comp, robust));
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return -3;
     cudaLaunchConfig_t cfg{};
@@ -870,11 +944,13 @@ static int fits_round(int C, int M, bool server_opt) {
 }
 
 // 1 when the fused kernel can run this federation: instantiated shape, t_cur < kTmax, shared-memory layout (with the server
-// optimizer state when server_opt) within 227 KB
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt) {
+// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule 2·C ≤ 33·P (a slot's uploads and
+// their ranked copy fit the ranking warp's gbuf)
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, bool robust) {
     if (t_cur >= kTmax) return 0;
-#define FDB_CASE(K, I, H, O) \
-    if (kind == K && din == I && (K == 0 || hid == H) && dout == O) return fits_round<Mlp<K, I, H, O>>(C, M, server_opt);
+#define FDB_CASE(K, I, H, O)                                                                               \
+    if (kind == K && din == I && (K == 0 || hid == H) && dout == O)                                        \
+        return fits_round<Mlp<K, I, H, O>>(C, M, server_opt) && (!robust || 2 * C <= 33 * Mlp<K, I, H, O>::P);
     FDB_MLP_SHAPES(FDB_CASE)
 #undef FDB_CASE
     return 0;

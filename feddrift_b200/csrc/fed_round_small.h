@@ -48,7 +48,12 @@ struct RoundParams {
     // the rest in ef_res, before client_out, the defense and the average see it
     float* ef_res;
     int topk_k;
-    float* client_out;  // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
+    // cluster aggregation rule (0 = weighted mean): 1 coordinate-wise median, 2 trimmed mean dropping
+    // ⌊fl32(trim_ratio · n)⌋ values at each end, over the n uploads of a slot as published (after compression and the
+    // defense), each counted once (ops/reference.py robust_aggregate_slots_); the server optimizer then steps on θ − it
+    int agg_rule;
+    float trim_ratio;
+    float* client_out; // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs
     float* metrics;      // [rounds, C, 4]
@@ -90,7 +95,7 @@ struct SmallLaunchInfo {
 int fed_round_small_launch(int kind, int din, int hid, int dout, const RoundParams& p, int cluster, cudaStream_t stream,
                            SmallLaunchInfo* info);
 int fed_round_small_supported(int kind, int din, int hid, int dout);
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt);
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, bool robust);
 int mlp_eval_matrix_launch(int kind, int din, int hid, int dout, const float* theta, int theta_stride, int M, const float* X,
                            const int* Y, const int* nsamp, int C, int S, float* correct, float* loss, float* sqerr,
                            cudaStream_t stream);

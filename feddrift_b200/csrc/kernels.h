@@ -29,6 +29,12 @@ int qsgd_slots_launch(float* rows, const float* theta, long long t_stride, int M
 long long eftopk_scratch_words(int R, long long P);
 int eftopk_slots_launch(float* rows, const float* theta, long long t_stride, int M, float* res, const float* n,
                         const unsigned char* mask, int R, long long P, long long k, unsigned* scratch, cudaStream_t stream);
+// robust_agg.cu (K19): coordinate-wise median (median = 1) or trimmed mean (trim ratio beta) of the rows with n[c·M + m] > 0
+// of cp [C, M, P] into theta + m·t_stride for every slot with a participant; opt_kind != 0 steps each such slot with the
+// server optimizer (bias corrections from steps[m] + 1; the caller advances steps).  -2: C too large for the staging tile
+int robust_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, int C, int M, long long P,
+                            int median, float beta, int opt_kind, float lr, float momentum, float b1, float b2, float eps,
+                            float* s0, float* s1, const int* steps, const unsigned char* mask, cudaStream_t stream);
 // aggregate_peer.cu : multi-GPU reduce-scatter + apply + all-gather over NVLink peer memory (cooperative launch)
 int fedavg_reduce_apply_peer_launch(const float* cp, const int* cidx, const float* n, int C, int M, int P, int theta_stride, int world, int rank,
                                     const long long* part_ptrs, const long long* theta_ptrs, const long long* tot_ptrs,

@@ -66,6 +66,10 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--quantize_level", type=int, default=16, help="QSGD levels s, 1..65535 (s = 1: ternary)")
     a("--quantize_bucket", type=int, default=512, help="QSGD bucket size b (entries per scale), >= 1")
     a("--topk_ratio", type=float, default=0.01, help="eftopk: fraction ρ of the trainable entries kept, 0 < ρ <= 1")
+    # Byzantine-robust cluster aggregation (Yin et al., 2018): the coordinate-wise median or β-trimmed mean of the slot's
+    # uploads (after compression and the defense), each participant counted once, instead of the weighted average
+    a("--aggregation_rule", type=str, default="mean", choices=["mean", "median", "trimmed_mean"])
+    a("--trim_ratio", type=float, default=0.1, help="trimmed_mean: fraction β dropped at each end, 0 <= β < 0.5")
     # FedProx local training: every client step minimises CE + mu/2‖w − w_m‖², w_m the cluster model it received (0 = off)
     a("--fedprox_mu", type=float, default=0.0)
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)

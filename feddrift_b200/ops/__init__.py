@@ -19,6 +19,7 @@ Kernel map (SURVEY §2.9 numbering):
   K14 kd_kl_loss   K15 vfl_bce_grad   K16 group_norm   csrc/misc.cu
   K17 qsgd_slots_ (upload quantization)           csrc/compress.cu
   K18 eftopk_slots_ (top-k + error feedback)      csrc/sparsify.cu
+  K19 robust_aggregate_slots_ (median / trimmed mean)   csrc/robust_agg.cu
 """
 from __future__ import annotations
 
@@ -50,9 +51,14 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
 
 
 # ----------------------------------------------------------------------------- K1
-def cluster_aggregate_(theta, client_params, n, server_opt=None):
+def cluster_aggregate_(theta, client_params, n, server_opt=None, rule=None):
     """K1: θ_m ← weighted mean of ``client_params[:, m]`` for every slot with total weight > 0; returns the totals [M].
-    ``server_opt`` (``server_opt.SlotServerOpt``) then steps each such slot on θ_m − avg_m with its own state."""
+    ``server_opt`` (``server_opt.SlotServerOpt``) then steps each such slot on θ_m − avg_m with its own state.
+    ``rule`` = ``(aggregation_rule, trim_ratio)`` with rule 'median' or 'trimmed_mean' replaces the weighted mean by K19
+    (``robust_aggregate_slots_``: the participants n > 0 count once each) and returns the participant counts [M]; None or
+    'mean' is the weighted mean above."""
+    if rule is not None and rule[0] != "mean":
+        return robust_aggregate_slots_(theta, client_params, n, rule[0], rule[1], server_opt)
     if server_opt is not None:
         if native(theta, client_params):
             return server_opt.aggregate_native_(theta, client_params, n)
@@ -60,6 +66,32 @@ def cluster_aggregate_(theta, client_params, n, server_opt=None):
     if native(theta, client_params):
         return _ext.load().cluster_aggregate(theta, client_params.contiguous(), n.float().contiguous())
     return ref.cluster_aggregate_(theta, client_params, n)
+
+
+def robust_aggregate_slots_(theta, uploads, n, rule: str = "median", trim_ratio: float = 0.1, server_opt=None):
+    """K19: θ_m ← coordinate-wise median / trimmed mean of the uploads ``uploads[c, m]`` with ``n[c, m] > 0`` (each counted
+    once) for every slot with a participant; ``theta`` may be a padded bank.  ``server_opt`` (``server_opt.SlotServerOpt``)
+    then steps each such slot on θ_m − statistic and advances its counter.  See ``reference.robust_aggregate_slots_``;
+    returns the participant counts [M]."""
+    rule, beta = ref.aggregation_params(rule, trim_ratio)
+    if rule == "mean":
+        raise ValueError("robust_aggregate_slots_: rule must be median or trimmed_mean")
+    if native(theta, uploads):
+        rid = 1 if rule == "median" else 2
+        nn = n.float().contiguous()
+        if server_opt is None:
+            return _ext.load().robust_aggregate_slots(theta, uploads.contiguous(), nn, rid, beta, 0, 0.0, 0.0, 1e-8,
+                                                      None, None, None, None)
+        so = server_opt
+        return _ext.load().robust_aggregate_slots(theta, uploads.contiguous(), nn, rid, beta, so.kind, so.lr, so.momentum, so.eps,
+                                                  so.s0, so.s1, so.step, so._mask_u8)
+    if server_opt is None:
+        return ref.robust_aggregate_slots_(theta, uploads, n, rule, beta)
+    avg = theta.clone()
+    counts = ref.robust_aggregate_slots_(avg, uploads, n, rule, beta)
+    so = server_opt
+    ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
+    return counts
 
 
 def weighted_average(rows, weights, out=None):

@@ -220,6 +220,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     updated in place like the optimizer moments): at the same point every trained pair's local model goes through
     ``eftopk_slots_`` against the round-start θ with k = ``topk_k(ρ, P)``; ``client_out``, the defense and the average see
     the sparsified model.
+    ``aggregation_rule`` 'median'|'trimmed_mean' (absent or 'mean': the weighted average) with ``trim_ratio`` β (0.1,
+    validated whatever the rule by ``aggregation_params``): after compression and the defense, every slot with a
+    participant becomes ``robust_aggregate_slots_`` of its trained pairs' uploads (each counts once, the weights are
+    ignored) instead of the weighted average; the server optimizer then steps on θ_m − that statistic.
     ``fedprox_mu`` (absent or 0: off): every local
     step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
     (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
@@ -254,6 +258,7 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     ef_k = topk_k(ef_ratio, P) if (st.get("compression") or "none") == "eftopk" else 0
     if ef_k and st.get("ef_residual") is None:
         st["ef_residual"] = torch.zeros(C, M, P, dtype=torch.float32)
+    agg_rule, trim_ratio = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -322,8 +327,14 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
             robust_clip_slots_(up, theta, trained, def_bound, None, def_std, defense_seed(seed, rnd))
             locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
         avg = theta.clone() if sopt is not None else theta
+        if agg_rule != "mean" and locals_:   # robust rule: every participant counts once, the weights are ignored
+            up = torch.zeros(C, M, P, dtype=torch.float32)
+            trained = torch.zeros(C, M)
+            for (c, m), (p, _) in locals_.items():
+                up[c, m], trained[c, m] = p, 1.0
+            robust_aggregate_slots_(avg, up, trained, agg_rule, trim_ratio)
         for m in range(M):
-            if acc_w[m] <= 0:
+            if acc_w[m] <= 0 or agg_rule != "mean":
                 continue
             tot = np.float32(acc_w[m])
             out = torch.zeros(P, dtype=torch.float32)
@@ -678,6 +689,78 @@ def topk_upload_bits(P_train: int, P_other: int, k: int) -> int:
     P_train, P_other, k = int(P_train), int(P_other), int(k)
     P = P_train + P_other
     return k * (32 + max(P - 1, 0).bit_length()) + 32 * P_other
+
+
+AGGREGATION_RULES = ("mean", "median", "trimmed_mean")
+
+
+def aggregation_params(rule, trim_ratio) -> Tuple[str, float]:
+    """Validated ``(--aggregation_rule, --trim_ratio)``.  The rule is one of ``mean`` (weighted FedAvg), ``median`` or
+    ``trimmed_mean``; β is checked whatever the rule and must be a finite number with 0 ≤ β < 0.5.  Raises ``ValueError``."""
+    rule = "mean" if rule is None else rule
+    if rule not in AGGREGATION_RULES:
+        raise ValueError(f"aggregation_rule must be one of {', '.join(AGGREGATION_RULES)} (got {rule!r})")
+    msg = f"trim_ratio must be a number in [0, 0.5) (got {trim_ratio!r})"
+    if isinstance(trim_ratio, bool):
+        raise ValueError(msg)
+    try:
+        b = float(trim_ratio)
+    except (TypeError, ValueError):
+        raise ValueError(msg) from None
+    if not (math.isfinite(b) and 0.0 <= b < 0.5):
+        raise ValueError(msg)
+    return rule, b
+
+
+def trim_count(beta, n: int) -> int:
+    """Values ``trimmed_mean`` drops at EACH end of a column of ``n`` uploads: ⌊fl32(fl32(β)·n)⌋, one fp32 rounding of the
+    product (``np.float32(β) * np.float32(n)``), so CPU and GPU agree.  β < 0.5 keeps at least one value."""
+    return int(np.floor(np.float32(beta) * np.float32(int(n))))
+
+
+_QNAN32 = np.uint32(0x7FC00000).view(np.float32).item()   # the NaN a column containing a NaN yields (GPU: same bits)
+
+
+def robust_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch.Tensor, rule: str = "median",
+                            trim_ratio: float = 0.1) -> torch.Tensor:
+    """Coordinate-wise robust aggregation (K19), in place: for every slot m, the participants are the rows c with
+    ``n[c, m] > 0`` (n of them; the weights are otherwise ignored: each participant counts once, so a client cannot buy
+    influence by reporting a large sample count).  For each entry e of ``theta[m, :P]`` (``theta`` may be a padded bank;
+    every entry, BatchNorm statistics included):
+
+    * the rank of upload i is #{j : a_j < a_i} + #{j < i : a_j == a_i}, compared as floats (−0 and +0 tie);
+    * ``median`` keeps ranks b … n−1−b with b = ⌊(n − 1)/2⌋, ``trimmed_mean`` with b = ``trim_count(β, n)``;
+    * the value is the fp32 sum of the kept values in ascending rank order, starting from the smallest kept one, then one
+      round-to-nearest division by (n − 2b); a column that holds a NaN yields NaN.
+
+    The result depends only on the multiset of uploads (any client permutation gives the same bits).  Slots with n = 0
+    keep θ_m.  Returns the per-slot participant counts ``[M]`` (float32)."""
+    rule, beta = aggregation_params(rule, trim_ratio)
+    if rule == "mean":
+        raise ValueError("robust_aggregate_slots_: the mean rule is the weighted average (cluster_aggregate_)")
+    C, M, P = uploads.shape
+    part = n.detach().reshape(C, M).to(uploads.device) > 0
+    counts = part.sum(0).to(torch.float32)
+    chunk = 1 << 20
+    for m in range(M):
+        idx = part[:, m].nonzero().flatten()
+        k = int(idx.numel())
+        if k == 0:
+            continue
+        b = (k - 1) // 2 if rule == "median" else trim_count(beta, k)
+        div = torch.tensor(float(k - 2 * b), dtype=torch.float32, device=uploads.device)
+        for e0 in range(0, P, chunk):
+            vals = uploads[idx, m, e0:e0 + chunk].to(torch.float32)
+            # stable ascending sort on +0-canonicalised keys: equal values (−0 and +0 included) stay in client order
+            order = torch.sort(vals + 0.0, dim=0, stable=True).indices
+            srt = torch.gather(vals, 0, order)
+            acc = srt[b].clone()
+            for j in range(b + 1, k - b):
+                acc = acc + srt[j]
+            out = acc / div
+            out = torch.where(torch.isnan(vals).any(0), torch.full_like(out, _QNAN32), out)
+            theta[m, e0:e0 + out.shape[0]] = out.to(theta.device)
+    return counts.to(theta.device)
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

@@ -11,6 +11,7 @@ from . import _ext
 
 KIND_ID = {"lr": 0, "fnn": 1}
 MODE_ID = {"pool": 0, "time": 1, "index": 2}
+AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2}
 LAUNCH_COUNT = {"fed_round_small": 0}
 
 
@@ -19,14 +20,17 @@ def supported(kind: str, din: int, hid: int, dout: int) -> bool:
     return ext is not None and bool(ext.fed_round_small_supported(KIND_ID[kind], din, hid, dout))
 
 
-def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, server_opt: bool = False) -> bool:
+def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, server_opt: bool = False,
+         robust: bool = False) -> bool:
     """True when the fused kernel can run this federation at time step ``t_cur`` (instantiated MLP shape, ``t_cur`` below
     the kernel's plan-table limit, shared-memory layout — plus the ``[2, M, P]`` server optimizer state when
-    ``server_opt`` — within 227 KB); otherwise route to the generic executor."""
+    ``server_opt`` — within 227 KB, and with a ``robust`` aggregation rule 2·C ≤ 33·P for the ranking scratch);
+    otherwise route to the generic executor."""
     ext = _ext.load()
     if ext is None:
         return True   # CPU reference has no such limits
-    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt)))
+    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt),
+                                         bool(robust)))
 
 
 def spin_timeout_ms(st: Dict) -> int:
@@ -158,6 +162,13 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
     elif compression != "none":
         from .reference import compression_params
         compression_params(compression, 16, 512)   # raises for an unknown compression
+    from .reference import aggregation_params
+    rule, beta = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
+    if rule != "mean":   # robust aggregation rule (reference.fed_round_small documents the keys)
+        if mg:
+            raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only")
+        fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer ... top-k slots, unread when off
+        fcfg += [float(AGG_RULE_ID[rule]), beta]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out

@@ -36,8 +36,8 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import (compression_params, prox_mu_param, qsgd_upload_bits, topk_k, topk_ratio_param,
-                             topk_upload_bits)
+from ..ops.reference import (aggregation_params, compression_params, prox_mu_param, qsgd_upload_bits, topk_k,
+                             topk_ratio_param, topk_upload_bits)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -54,6 +54,7 @@ DEFAULTS = dict(
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
     compression="none", quantize_level=16, quantize_bucket=512, topk_ratio=0.01,
+    aggregation_rule="mean", trim_ratio=0.1,
 )
 
 
@@ -112,6 +113,10 @@ class DriftSim:
         self.topk_ratio = topk_ratio_param(getattr(args, "topk_ratio", 0.01))
         n_train = int(wmask[: self.bank.P].sum())
         self.topk_k = topk_k(self.topk_ratio, n_train) if (getattr(args, "compression", "none") or "none") == "eftopk" else 0
+        # cluster aggregation rule (--aggregation_rule / --trim_ratio): 'mean' is the weighted FedAvg average; a robust rule
+        # replaces it by the coordinate-wise median / trimmed mean of the slot's uploads (agg_rule = (rule, β), None = mean)
+        rule, beta = aggregation_params(getattr(args, "aggregation_rule", "mean") or "mean", getattr(args, "trim_ratio", 0.1))
+        self.agg_rule = None if rule == "mean" else (rule, beta)
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -238,6 +243,8 @@ class DriftSim:
                 self._small.update(compression="qsgd", quantize_level=self.q_level, quantize_bucket=self.q_bucket)
             if self.topk_k:   # the arena's residual: the kernel reads and writes it in place
                 self._small.update(compression="eftopk", topk_ratio=self.topk_ratio, ef_residual=self.clients.ef_res)
+            if self.agg_rule is not None:
+                self._small.update(aggregation_rule=self.agg_rule[0], trim_ratio=self.agg_rule[1])
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)
@@ -254,6 +261,9 @@ class DriftSim:
         if self.bank.server_opt is not None and (self.multi is not None or getattr(self, "shard_clients", False)):
             raise ValueError("a server optimizer (--server_optimizer) is single-GPU only: it cannot be combined with "
                              "multi-GPU client sharding")
+        if self.agg_rule is not None and (self.multi is not None or getattr(self, "shard_clients", False)):
+            raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only: an order statistic needs every "
+                             "upload on one device, so it cannot be combined with multi-GPU client sharding")
         done, last = 0, {}
         while done < rounds:
             block = self.algo.block_size(self.round_in_step, rounds - done)
@@ -289,7 +299,7 @@ class DriftSim:
         from ..ops import small_round
         s = self.spec
         return small_round.fits(s["kind"], s["in"], s["hidden"], s["out"], self.C, self.M, self.t,
-                                server_opt=self.bank.server_opt is not None)
+                                server_opt=self.bank.server_opt is not None, robust=self.agg_rule is not None)
 
     def upload_bits(self) -> int:
         """Size in bits of one compressed upload of this federation (``reference.qsgd_upload_bits`` under QSGD,
