@@ -136,6 +136,88 @@ FDB_DEVICE void robust_columns(float* slot_s, const int* pairs_s, int npairs, co
     }
 }
 
+// Geometric-median phase (RoundParams::agg_rule == 3), after robust_columns has left the coordinate-wise median of the
+// columns e ≡ crank (mod G) in every CTA's part and a cluster barrier: CTA crank refines each slot m ≡ crank (mod G) with
+// `iters` smoothed Weiszfeld steps (ops/reference.py geomed_aggregate_slots_) and leaves v_m in its own part[m·P …] (only
+// the slot's owner reads those entries of it).  v⁰ comes from the column owners; the slot's n uploads are copied over DSMEM
+// in pair order into scratch [n][P], followed by the weights [n], the pair list [n] and {W, n, NaN flag} — the CTA's gbuf,
+// free after the ranking (fed_round_small_fits checks C·(P + 2) + 4 floats fit).  Warps over rows for the fp64 distances,
+// threads over columns for the update Σ fl32(w_i·x_i) / W, every operation rounded on its own as in the oracle.
+template <int P>
+__device__ __noinline__ void geomed_slots(const float* slot_s, const int* pairs_s, int npairs, const float* tot_s, float* part, float* scratch,
+                             int C, int M, int G, int crank, int warp, int NW, int lane, int iters, double nu) {
+    cg::cluster_group cluster = cg::this_cluster();
+    const int tid = threadIdx.x, nthreads = NW * 32;
+    float* X = scratch;
+    float* w = X + (size_t)C * P;
+    int* lst = reinterpret_cast<int*>(w + C);
+    float* Ws = reinterpret_cast<float*>(lst + C);
+    int* n_s = reinterpret_cast<int*>(Ws + 1);
+    int* nan_s = n_s + 1;
+    for (int m = crank; m < M; m += G) {
+        if (!(tot_s[m] > 0.f)) continue;
+        float* v = part + m * P;
+        if (warp == 0) {   // the slot's pairs in pair order
+            int base = 0;
+            for (int i0 = 0; i0 < npairs; i0 += 32) {
+                const int i = i0 + lane;
+                const bool on = i < npairs && pairs_s[i] % M == m;
+                const unsigned bal = __ballot_sync(0xffffffffu, on);
+                if (on) lst[base + __popc(bal & ((1u << lane) - 1u))] = i;
+                base += __popc(bal);
+            }
+            if (lane == 0) { *n_s = base; *nan_s = 0; }
+        }
+        for (int pp = tid; pp < P; pp += nthreads) v[pp] = *(cluster.map_shared_rank(part + m * P + pp, (m * P + pp) % G));
+        __syncthreads();
+        const int n = *n_s;
+        if (n > 2) {
+            for (int idx = tid; idx < n * P; idx += nthreads) {
+                const int i = idx / P, pp = idx - i * P, pi = lst[i];
+                X[idx] = *(cluster.map_shared_rank(slot_s + (pi / G) * P + pp, pi % G));
+            }
+            __syncthreads();
+            for (int it = 0; it < iters; ++it) {
+                for (int i = warp; i < n; i += NW) {
+                    double s = 0.0;
+                    for (int pp = lane; pp < P; pp += 32) {
+                        const double d = (double)__fsub_rn(X[i * P + pp], v[pp]);
+                        s = fma(d, d, s);
+                    }
+                    s = warp_sum(s);
+                    if (lane == 0) {
+                        if (isnan(s)) *nan_s = 1;
+                        w[i] = isnan(s) ? 0.f : (float)(1.0 / fmax(nu, sqrt(s)));
+                    }
+                }
+                __syncthreads();
+                if (tid == 0) {
+                    float W = 0.f;
+                    for (int i = 0; i < n; ++i) W = __fadd_rn(W, w[i]);
+                    *Ws = W;
+                }
+                __syncthreads();
+                const float W = *Ws;
+                if (*nan_s) {
+                    for (int pp = tid; pp < P; pp += nthreads) v[pp] = __int_as_float(0x7FC00000);
+                    break;
+                }
+                if (W == 0.f) break;   // keeps v
+                for (int pp = tid; pp < P; pp += nthreads) {
+                    float acc = 0.f;
+                    for (int i = 0; i < n; ++i) {
+                        const float wi = w[i];
+                        if (wi != 0.f) acc = __fadd_rn(acc, __fmul_rn(wi, X[i * P + pp]));
+                    }
+                    v[pp] = __fdiv_rn(acc, W);
+                }
+                __syncthreads();
+            }
+        }
+        __syncthreads();   // the next slot rewrites the scratch and the flags
+    }
+}
+
 // sample coordinates of element i of the current mini-batch
 struct BatchSel {
     int mode;        // 0/1: contiguous [lo, lo+n) of (tb, c);  2: list
@@ -149,7 +231,7 @@ constexpr int kCompNone = 0, kCompQsgd = 1, kCompEfTopk = 2;
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
 // its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kComp: the upload compression
 // (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0) and kRobust: a median / trimmed-mean aggregation rule
-// (p.agg_rule != 0), separate for the same reason
+// or geometric median (p.agg_rule != 0), separate for the same reason
 template <class Net, bool kDefend, bool kProx, int kComp, bool kRobust>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
@@ -612,7 +694,12 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                 // lives in CTA i mod G, slot i / G; pairs_s is the same in every CTA), with the warp's gbuf as scratch
                 if (G > 1) cluster.sync(); else __syncthreads();
                 robust_columns<P>(slot_s, pairs_s, npairs, tot_s, theta_s, part_s + buf * MP, smem + L.gbuf + warp * (P * 33),
-                                  M, G, crank, warp, NW, lane, p.agg_rule == 1, p.trim_ratio);
+                                  M, G, crank, warp, NW, lane, p.agg_rule != 2, p.trim_ratio);
+                if (p.agg_rule == 3) {   // geometric median: start from that median, CTA k refines the slots m ≡ k (mod G)
+                    if (G > 1) cluster.sync(); else __syncthreads();
+                    geomed_slots<P>(slot_s, pairs_s, npairs, tot_s, part_s + buf * MP, smem + L.gbuf, C, M, G, crank, warp, NW, lane,
+                                    p.gm_iters, p.gm_nu);
+                }
             }
             if (G > 1) cluster.sync(); else __syncthreads();
             if (p.world == 1) {
@@ -620,7 +707,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     const int m = e / P;
                     if (tot_s[m] > 0.f) {
                         float v = 0.f;
-                        if constexpr (kRobust) v = *(cluster.map_shared_rank(part_s + buf * MP + e, e % G));   // the column's owner
+                        if constexpr (kRobust)   // the column's owner (geometric median: the slot's owner)
+                            v = *(cluster.map_shared_rank(part_s + buf * MP + e, p.agg_rule == 3 ? m % G : e % G));
                         else for (int rk = 0; rk < G; ++rk) v += *(cluster.map_shared_rank(part_s + buf * MP + e, rk));
                         if (p.sopt_kind) {
                             const float ts = (float)(sstep_s[m] + 1);
@@ -944,13 +1032,16 @@ static int fits_round(int C, int M, bool server_opt) {
 }
 
 // 1 when the fused kernel can run this federation: instantiated shape, t_cur < kTmax, shared-memory layout (with the server
-// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule 2·C ≤ 33·P (a slot's uploads and
-// their ranked copy fit the ranking warp's gbuf)
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, bool robust) {
+// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule (agg_rule 1..3) 2·C ≤ 33·P (a slot's
+// uploads and their ranked copy fit the ranking warp's gbuf); the geometric median (3) also needs C·(P + 2) + 4 ≤ the
+// CTA's gbuf (a slot's uploads, weights and pair list)
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule) {
     if (t_cur >= kTmax) return 0;
-#define FDB_CASE(K, I, H, O)                                                                               \
-    if (kind == K && din == I && (K == 0 || hid == H) && dout == O)                                        \
-        return fits_round<Mlp<K, I, H, O>>(C, M, server_opt) && (!robust || 2 * C <= 33 * Mlp<K, I, H, O>::P);
+#define FDB_CASE(K, I, H, O)                                                                                            \
+    if (kind == K && din == I && (K == 0 || hid == H) && dout == O)                                                     \
+        return fits_round<Mlp<K, I, H, O>>(C, M, server_opt) && (agg_rule == 0 || 2 * C <= 33 * Mlp<K, I, H, O>::P) && \
+               (agg_rule != 3 || (long long)C * (Mlp<K, I, H, O>::P + 2) + 4 <=                                          \
+                                     (long long)SmallCfg<Mlp<K, I, H, O>>::kWarps * 33 * Mlp<K, I, H, O>::P);
     FDB_MLP_SHAPES(FDB_CASE)
 #undef FDB_CASE
     return 0;

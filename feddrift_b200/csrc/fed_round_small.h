@@ -53,6 +53,10 @@ struct RoundParams {
     // defense), each counted once (ops/reference.py robust_aggregate_slots_); the server optimizer then steps on θ − it
     int agg_rule;
     float trim_ratio;
+    // agg_rule 3: geometric median (ops/reference.py geomed_aggregate_slots_): gm_iters smoothed Weiszfeld steps from the
+    // coordinate-wise median, weights 1 / max(gm_nu, distance)
+    int gm_iters;
+    double gm_nu;
     float* client_out; // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs
@@ -95,7 +99,7 @@ struct SmallLaunchInfo {
 int fed_round_small_launch(int kind, int din, int hid, int dout, const RoundParams& p, int cluster, cudaStream_t stream,
                            SmallLaunchInfo* info);
 int fed_round_small_supported(int kind, int din, int hid, int dout);
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, bool robust);
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule);
 int mlp_eval_matrix_launch(int kind, int din, int hid, int dout, const float* theta, int theta_stride, int M, const float* X,
                            const int* Y, const int* nsamp, int C, int S, float* correct, float* loss, float* sqerr,
                            cudaStream_t stream);

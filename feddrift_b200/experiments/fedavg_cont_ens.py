@@ -68,8 +68,11 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--topk_ratio", type=float, default=0.01, help="eftopk: fraction ρ of the trainable entries kept, 0 < ρ <= 1")
     # Byzantine-robust cluster aggregation (Yin et al., 2018): the coordinate-wise median or β-trimmed mean of the slot's
     # uploads (after compression and the defense), each participant counted once, instead of the weighted average
-    a("--aggregation_rule", type=str, default="mean", choices=["mean", "median", "trimmed_mean"])
+    a("--aggregation_rule", type=str, default="mean", choices=["mean", "median", "trimmed_mean", "geometric_median"])
     a("--trim_ratio", type=float, default=0.1, help="trimmed_mean: fraction β dropped at each end, 0 <= β < 0.5")
+    # geometric median (RFA, Pillutla et al.): smoothed Weiszfeld steps from the coordinate-wise median
+    a("--geomed_iters", type=int, default=4, help="geometric_median: Weiszfeld iterations R, 1..100")
+    a("--geomed_nu", type=float, default=1e-6, help="geometric_median: smoothing ν > 0 (weights 1 / max(ν, distance))")
     # FedProx local training: every client step minimises CE + mu/2‖w − w_m‖², w_m the cluster model it received (0 = off)
     a("--fedprox_mu", type=float, default=0.0)
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)

@@ -20,6 +20,7 @@ Kernel map (SURVEY §2.9 numbering):
   K17 qsgd_slots_ (upload quantization)           csrc/compress.cu
   K18 eftopk_slots_ (top-k + error feedback)      csrc/sparsify.cu
   K19 robust_aggregate_slots_ (median / trimmed mean)   csrc/robust_agg.cu
+  K20 geomed_aggregate_slots_ (geometric median)        csrc/robust_agg.cu
 """
 from __future__ import annotations
 
@@ -51,12 +52,15 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
 
 
 # ----------------------------------------------------------------------------- K1
-def cluster_aggregate_(theta, client_params, n, server_opt=None, rule=None):
+def cluster_aggregate_(theta, client_params, n, server_opt=None, rule=None, mask=None):
     """K1: θ_m ← weighted mean of ``client_params[:, m]`` for every slot with total weight > 0; returns the totals [M].
     ``server_opt`` (``server_opt.SlotServerOpt``) then steps each such slot on θ_m − avg_m with its own state.
     ``rule`` = ``(aggregation_rule, trim_ratio)`` with rule 'median' or 'trimmed_mean' replaces the weighted mean by K19
     (``robust_aggregate_slots_``: the participants n > 0 count once each) and returns the participant counts [M]; None or
-    'mean' is the weighted mean above."""
+    'mean' is the weighted mean above.  ``rule`` = ``('geometric_median', trim_ratio, iters, nu)`` takes K20
+    (``geomed_aggregate_slots_``) instead, with ``mask`` the trainable entries its distances cover (None: all)."""
+    if rule is not None and rule[0] == "geometric_median":
+        return geomed_aggregate_slots_(theta, client_params, n, rule[2], rule[3], server_opt, mask)
     if rule is not None and rule[0] != "mean":
         return robust_aggregate_slots_(theta, client_params, n, rule[0], rule[1], server_opt)
     if server_opt is not None:
@@ -74,7 +78,7 @@ def robust_aggregate_slots_(theta, uploads, n, rule: str = "median", trim_ratio:
     then steps each such slot on θ_m − statistic and advances its counter.  See ``reference.robust_aggregate_slots_``;
     returns the participant counts [M]."""
     rule, beta = ref.aggregation_params(rule, trim_ratio)
-    if rule == "mean":
+    if rule not in ("median", "trimmed_mean"):
         raise ValueError("robust_aggregate_slots_: rule must be median or trimmed_mean")
     if native(theta, uploads):
         rid = 1 if rule == "median" else 2
@@ -89,6 +93,31 @@ def robust_aggregate_slots_(theta, uploads, n, rule: str = "median", trim_ratio:
         return ref.robust_aggregate_slots_(theta, uploads, n, rule, beta)
     avg = theta.clone()
     counts = ref.robust_aggregate_slots_(avg, uploads, n, rule, beta)
+    so = server_opt
+    ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
+    return counts
+
+
+def geomed_aggregate_slots_(theta, uploads, n, iters: int = 4, nu: float = 1e-6, server_opt=None, mask=None):
+    """K20: θ_m ← geometric median (``iters`` smoothed Weiszfeld steps from the coordinate-wise median, smoothing ``nu``) of
+    the uploads ``uploads[c, m]`` with ``n[c, m] > 0`` (each counted once) for every slot with a participant; ``theta`` may be
+    a padded bank; ``mask`` [P] (bool, None = all) selects the entries of the distances (BatchNorm statistics are
+    aggregated but left out).  ``server_opt`` then steps each such slot on θ_m − v and advances its counter.  See
+    ``reference.geomed_aggregate_slots_``; returns the participant counts [M]."""
+    iters, nu = ref.geomed_params(iters, nu)
+    if native(theta, uploads):
+        nn = n.float().contiguous()
+        dm = None if mask is None else mask.reshape(-1)[: uploads.shape[2]].to(uploads.device, torch.uint8).contiguous()
+        if server_opt is None:
+            return _ext.load().geomed_aggregate_slots(theta, uploads.contiguous(), nn, iters, nu, 0, 0.0, 0.0, 1e-8,
+                                                      None, None, None, None, dm)
+        so = server_opt
+        return _ext.load().geomed_aggregate_slots(theta, uploads.contiguous(), nn, iters, nu, so.kind, so.lr, so.momentum, so.eps,
+                                                  so.s0, so.s1, so.step, so._mask_u8, dm)
+    if server_opt is None:
+        return ref.geomed_aggregate_slots_(theta, uploads, n, iters, nu, mask)
+    avg = theta.clone()
+    counts = ref.geomed_aggregate_slots_(avg, uploads, n, iters, nu, mask)
     so = server_opt
     ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
     return counts

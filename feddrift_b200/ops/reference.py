@@ -6,7 +6,7 @@ compare the sm_90a kernels against.  Nothing here is tuned; clarity wins.
 from __future__ import annotations
 
 import math
-from typing import Dict, Tuple
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
@@ -224,6 +224,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     validated whatever the rule by ``aggregation_params``): after compression and the defense, every slot with a
     participant becomes ``robust_aggregate_slots_`` of its trained pairs' uploads (each counts once, the weights are
     ignored) instead of the weighted average; the server optimizer then steps on θ_m − that statistic.
+    ``aggregation_rule`` 'geometric_median' with ``geomed_iters`` R (4) and ``geomed_nu`` ν (1e-6), validated whatever the
+    rule by ``geomed_params``: the same, with ``geomed_aggregate_slots_`` (every entry is trainable in these MLPs).
     ``fedprox_mu`` (absent or 0: off): every local
     step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
     (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
@@ -259,6 +261,7 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     if ef_k and st.get("ef_residual") is None:
         st["ef_residual"] = torch.zeros(C, M, P, dtype=torch.float32)
     agg_rule, trim_ratio = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
+    gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -332,7 +335,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
             trained = torch.zeros(C, M)
             for (c, m), (p, _) in locals_.items():
                 up[c, m], trained[c, m] = p, 1.0
-            robust_aggregate_slots_(avg, up, trained, agg_rule, trim_ratio)
+            if agg_rule == "geometric_median":
+                geomed_aggregate_slots_(avg, up, trained, gm_iters, gm_nu)
+            else:
+                robust_aggregate_slots_(avg, up, trained, agg_rule, trim_ratio)
         for m in range(M):
             if acc_w[m] <= 0 or agg_rule != "mean":
                 continue
@@ -691,12 +697,13 @@ def topk_upload_bits(P_train: int, P_other: int, k: int) -> int:
     return k * (32 + max(P - 1, 0).bit_length()) + 32 * P_other
 
 
-AGGREGATION_RULES = ("mean", "median", "trimmed_mean")
+AGGREGATION_RULES = ("mean", "median", "trimmed_mean", "geometric_median")
 
 
 def aggregation_params(rule, trim_ratio) -> Tuple[str, float]:
-    """Validated ``(--aggregation_rule, --trim_ratio)``.  The rule is one of ``mean`` (weighted FedAvg), ``median`` or
-    ``trimmed_mean``; β is checked whatever the rule and must be a finite number with 0 ≤ β < 0.5.  Raises ``ValueError``."""
+    """Validated ``(--aggregation_rule, --trim_ratio)``.  The rule is one of ``mean`` (weighted FedAvg), ``median``,
+    ``trimmed_mean`` or ``geometric_median``; β is checked whatever the rule and must be a finite number with 0 ≤ β < 0.5.
+    Raises ``ValueError``."""
     rule = "mean" if rule is None else rule
     if rule not in AGGREGATION_RULES:
         raise ValueError(f"aggregation_rule must be one of {', '.join(AGGREGATION_RULES)} (got {rule!r})")
@@ -736,8 +743,9 @@ def robust_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch
     The result depends only on the multiset of uploads (any client permutation gives the same bits).  Slots with n = 0
     keep θ_m.  Returns the per-slot participant counts ``[M]`` (float32)."""
     rule, beta = aggregation_params(rule, trim_ratio)
-    if rule == "mean":
-        raise ValueError("robust_aggregate_slots_: the mean rule is the weighted average (cluster_aggregate_)")
+    if rule not in ("median", "trimmed_mean"):
+        raise ValueError("robust_aggregate_slots_: rule must be median or trimmed_mean (the mean is cluster_aggregate_, the "
+                         "geometric median geomed_aggregate_slots_)")
     C, M, P = uploads.shape
     part = n.detach().reshape(C, M).to(uploads.device) > 0
     counts = part.sum(0).to(torch.float32)
@@ -761,6 +769,88 @@ def robust_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch
             out = torch.where(torch.isnan(vals).any(0), torch.full_like(out, _QNAN32), out)
             theta[m, e0:e0 + out.shape[0]] = out.to(theta.device)
     return counts.to(theta.device)
+
+
+GEOMED_MAX_ITERS = 100
+
+
+def geomed_params(iters, nu) -> Tuple[int, float]:
+    """Validated ``(--geomed_iters, --geomed_nu)``, checked whatever the rule: R an int with 1 ≤ R ≤ 100 (a bool is not
+    an int here), ν a finite number > 0.  Raises ``ValueError``."""
+    if isinstance(iters, bool) or not isinstance(iters, (int, np.integer)) or not 1 <= int(iters) <= GEOMED_MAX_ITERS:
+        raise ValueError(f"geomed_iters must be an int in [1, {GEOMED_MAX_ITERS}] (got {iters!r})")
+    msg = f"geomed_nu must be a finite number > 0 (got {nu!r})"
+    if isinstance(nu, bool):
+        raise ValueError(msg)
+    try:
+        v = float(nu)
+    except (TypeError, ValueError):
+        raise ValueError(msg) from None
+    if not (math.isfinite(v) and v > 0.0):
+        raise ValueError(msg)
+    return int(iters), v
+
+
+def geomed_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch.Tensor, iters: int = 4, nu: float = 1e-6,
+                            mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Geometric median (K20, RFA's smoothed Weiszfeld iteration), in place.  For every slot m the participants x_1…x_n are
+    the rows c with ``n[c, m] > 0`` in ascending c, each counted once (the weights are ignored, as in
+    ``robust_aggregate_slots_``); ``theta`` may be a padded bank.
+
+    * Start: v⁰ = the coordinate-wise median (``robust_aggregate_slots_(…, "median")``).  With n ≤ 2 that is the result.
+    * Iteration t = 1…R (R = ``iters``):
+      d_i² = Σ_e mask_e · (double) fl32(x_ie − v_e)², the fp32 difference squared and summed in float64 (``mask``: the
+      trainable entries, None = all, so BatchNorm statistics stay out of the distance);
+      w_i = fl32(1 / max(ν, √d_i²)) computed in float64 and rounded once (d_i = +∞ gives w_i = 0: the row is left out);
+      W = the fp32 sum of the w_i in client order;
+      v_e = fl32(Σ_i fl32(w_i · x_ie)) summed in client order from 0 over the rows with w_i ≠ 0, then one round-to-nearest
+      division by W, for every entry (BatchNorm statistics included).
+    * W = 0 keeps the current v (and every later iteration would too).  A NaN distance makes the slot NaN (0x7FC00000)
+      in every entry.
+
+    The float64 distance sums depend on the reduction order, so the GPU matches this to a tolerance; given identical
+    weights the update is bit-exact.  Slots with n = 0 keep θ_m.  Returns the per-slot participant counts ``[M]``."""
+    R, nu = geomed_params(iters, nu)
+    counts = robust_aggregate_slots_(theta, uploads, n, "median")
+    C, M, P = uploads.shape
+    dev = uploads.device
+    part = n.detach().reshape(C, M).to(dev) > 0
+    keep = None if mask is None else mask.reshape(-1)[:P].to(dev, torch.bool)
+    chunk = 1 << 20
+    for m in range(M):
+        idx = part[:, m].nonzero().flatten().tolist()
+        k = len(idx)
+        if k <= 2:
+            continue
+        v = theta[m, :P].to(dev, torch.float32).clone()
+        for _ in range(R):
+            d2 = torch.zeros(k, dtype=torch.float64, device=dev)
+            for e0 in range(0, P, chunk):
+                diff = (uploads[idx, m, e0:e0 + chunk].to(torch.float32) - v[e0:e0 + chunk]).double()
+                sq = diff * diff
+                if keep is not None:
+                    sq = torch.where(keep[e0:e0 + chunk], sq, torch.zeros((), dtype=torch.float64, device=dev))
+                d2 += sq.sum(1)
+            if bool(torch.isnan(d2).any()):
+                v.fill_(_QNAN32)
+                break
+            w = (1.0 / torch.clamp(torch.sqrt(d2), min=nu)).to(torch.float32)
+            W = np.float32(0.0)
+            for wi in w.tolist():
+                W = np.float32(W + np.float32(wi))
+            if W == 0:
+                break
+            rows = [i for i in range(k) if float(w[i]) != 0.0]
+            div = torch.tensor(float(W), dtype=torch.float32, device=dev)
+            new = torch.empty_like(v)
+            for e0 in range(0, P, chunk):
+                acc = torch.zeros(min(chunk, P - e0), dtype=torch.float32, device=dev)
+                for i in rows:
+                    acc = acc + w[i] * uploads[idx[i], m, e0:e0 + chunk].to(torch.float32)
+                new[e0:e0 + chunk] = acc / div
+            v = new
+        theta[m, :P] = v.to(theta.device)
+    return counts
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

@@ -11,7 +11,7 @@ from . import _ext
 
 KIND_ID = {"lr": 0, "fnn": 1}
 MODE_ID = {"pool": 0, "time": 1, "index": 2}
-AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2}
+AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2, "geometric_median": 3}
 LAUNCH_COUNT = {"fed_round_small": 0}
 
 
@@ -21,16 +21,17 @@ def supported(kind: str, din: int, hid: int, dout: int) -> bool:
 
 
 def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, server_opt: bool = False,
-         robust: bool = False) -> bool:
+         robust: bool = False, rule: Optional[str] = None) -> bool:
     """True when the fused kernel can run this federation at time step ``t_cur`` (instantiated MLP shape, ``t_cur`` below
     the kernel's plan-table limit, shared-memory layout — plus the ``[2, M, P]`` server optimizer state when
-    ``server_opt`` — within 227 KB, and with a ``robust`` aggregation rule 2·C ≤ 33·P for the ranking scratch);
+    ``server_opt`` — within 227 KB, and with a ``robust`` aggregation rule 2·C ≤ 33·P for the ranking scratch; ``rule``
+    'geometric_median' (implies ``robust``) also needs a slot's C uploads and weights in the CTA's gradient buffers);
     otherwise route to the generic executor."""
     ext = _ext.load()
     if ext is None:
         return True   # CPU reference has no such limits
-    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt),
-                                         bool(robust)))
+    rid = AGG_RULE_ID[rule] if rule not in (None, "mean") else (1 if robust else 0)
+    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt), rid))
 
 
 def spin_timeout_ms(st: Dict) -> int:
@@ -162,13 +163,16 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
     elif compression != "none":
         from .reference import compression_params
         compression_params(compression, 16, 512)   # raises for an unknown compression
-    from .reference import aggregation_params
+    from .reference import aggregation_params, geomed_params
     rule, beta = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
+    gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
     if rule != "mean":   # robust aggregation rule (reference.fed_round_small documents the keys)
         if mg:
             raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only")
         fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0][len(fcfg) - 5:]   # server optimizer ... top-k slots, unread when off
         fcfg += [float(AGG_RULE_ID[rule]), beta]
+        if rule == "geometric_median":
+            fcfg += [float(gm_iters), gm_nu]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out

@@ -36,8 +36,8 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, compression_params, prox_mu_param, qsgd_upload_bits, topk_k,
-                             topk_ratio_param, topk_upload_bits)
+from ..ops.reference import (aggregation_params, compression_params, geomed_params, prox_mu_param, qsgd_upload_bits,
+                             topk_k, topk_ratio_param, topk_upload_bits)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -54,7 +54,7 @@ DEFAULTS = dict(
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
     compression="none", quantize_level=16, quantize_bucket=512, topk_ratio=0.01,
-    aggregation_rule="mean", trim_ratio=0.1,
+    aggregation_rule="mean", trim_ratio=0.1, geomed_iters=4, geomed_nu=1e-6,
 )
 
 
@@ -116,7 +116,9 @@ class DriftSim:
         # cluster aggregation rule (--aggregation_rule / --trim_ratio): 'mean' is the weighted FedAvg average; a robust rule
         # replaces it by the coordinate-wise median / trimmed mean of the slot's uploads (agg_rule = (rule, β), None = mean)
         rule, beta = aggregation_params(getattr(args, "aggregation_rule", "mean") or "mean", getattr(args, "trim_ratio", 0.1))
-        self.agg_rule = None if rule == "mean" else (rule, beta)
+        # the geometric median (--geomed_iters R / --geomed_nu ν, validated whatever the rule) carries (rule, β, R, ν)
+        gm_iters, gm_nu = geomed_params(getattr(args, "geomed_iters", 4), getattr(args, "geomed_nu", 1e-6))
+        self.agg_rule = None if rule == "mean" else ((rule, beta, gm_iters, gm_nu) if rule == "geometric_median" else (rule, beta))
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -245,6 +247,8 @@ class DriftSim:
                 self._small.update(compression="eftopk", topk_ratio=self.topk_ratio, ef_residual=self.clients.ef_res)
             if self.agg_rule is not None:
                 self._small.update(aggregation_rule=self.agg_rule[0], trim_ratio=self.agg_rule[1])
+                if self.agg_rule[0] == "geometric_median":
+                    self._small.update(geomed_iters=self.agg_rule[2], geomed_nu=self.agg_rule[3])
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)
@@ -299,7 +303,8 @@ class DriftSim:
         from ..ops import small_round
         s = self.spec
         return small_round.fits(s["kind"], s["in"], s["hidden"], s["out"], self.C, self.M, self.t,
-                                server_opt=self.bank.server_opt is not None, robust=self.agg_rule is not None)
+                                server_opt=self.bank.server_opt is not None, robust=self.agg_rule is not None,
+                                rule=None if self.agg_rule is None else self.agg_rule[0])
 
     def upload_bits(self) -> int:
         """Size in bits of one compressed upload of this federation (``reference.qsgd_upload_bits`` under QSGD,

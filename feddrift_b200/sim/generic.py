@@ -14,7 +14,8 @@ architecture and for algorithms that must look at raw client updates before aggr
   (``ops.robust_clip_slots_``, K10) after the raw-update hooks have seen them; QSGD upload compression quantizes the
   trained rows in place (``ops.qsgd_slots_``, K17) right after local training, so the hooks see the quantized uploads;
   top-k with error feedback sparsifies them there instead (``ops.eftopk_slots_``, K18, residual ``ClientArena.ef_res``);
-  a robust aggregation rule (``sim.agg_rule``) makes the same call take the coordinate-wise median / trimmed mean (K19);
+  a robust aggregation rule (``sim.agg_rule``) makes the same call take the coordinate-wise median / trimmed mean (K19)
+  or the geometric median (K20, distances over the trainable entries ``sim.defense_mask``);
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -143,7 +144,11 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
             if world > 1:
                 _peer_aggregate(sim, world, rank)
             else:
-                ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, getattr(sim, "agg_rule", None))
+                rule = getattr(sim, "agg_rule", None)
+                if rule is not None and rule[0] == "geometric_median":
+                    ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule, mask=sim.defense_mask)
+                else:
+                    ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule)
         if plan.get("recluster_hard"):
             acc = sim.evaluator.acc_matrix(list(range(M)), t)
             best = np.argmax(acc, axis=0)
