@@ -152,10 +152,12 @@ std::vector<int64_t> fed_round_small(
             p.ef_res = er.data_ptr<float>();
         }
     }
-    if (fcfg.size() >= 16) {   // aggregation rule: fcfg[14] = 0 mean / 1 median / 2 trimmed mean / 3 geometric median, fcfg[15] = trim ratio
+    if (fcfg.size() >= 16) {   // aggregation rule: fcfg[14] = 0 mean / 1 median / 2 trimmed mean / 3 geometric median / 4 Multi-Krum,
+                               // fcfg[15] = trim ratio
         const double rule = fcfg[14], beta = fcfg[15];
-        TORCH_CHECK(rule == 0.0 || rule == 1.0 || rule == 2.0 || rule == 3.0,
-                    "fed_round_small: aggregation rule must be 0 (mean), 1 (median), 2 (trimmed_mean) or 3 (geometric_median)");
+        TORCH_CHECK(rule == 0.0 || rule == 1.0 || rule == 2.0 || rule == 3.0 || rule == 4.0,
+                    "fed_round_small: aggregation rule must be 0 (mean), 1 (median), 2 (trimmed_mean), 3 (geometric_median) or 4 "
+                    "(multi_krum)");
         TORCH_CHECK(std::isfinite(beta) && beta >= 0.0 && beta < 0.5, "fed_round_small: trim_ratio must be in [0, 0.5)");
         p.agg_rule = (int)rule; p.trim_ratio = (float)beta;
         if (p.agg_rule == 3) {   // fcfg[16] = Weiszfeld iterations R, fcfg[17] = smoothing nu
@@ -165,12 +167,22 @@ std::vector<int64_t> fed_round_small(
             TORCH_CHECK(std::isfinite(fcfg[17]) && fcfg[17] > 0.0, "fed_round_small: geomed_nu must be finite and > 0");
             p.gm_iters = (int)fcfg[16]; p.gm_nu = fcfg[17];
         }
+        if (p.agg_rule == 4) {   // fcfg[18] = Byzantine uploads f assumed per slot, fcfg[19] = uploads m averaged
+            TORCH_CHECK(fcfg.size() >= 20, "fed_round_small: Multi-Krum needs fcfg {.., geomed_iters, geomed_nu, krum_f, krum_m}");
+            TORCH_CHECK(fcfg[18] >= 0.0 && fcfg[18] <= 65535.0 && fcfg[18] == std::floor(fcfg[18]),
+                        "fed_round_small: krum_f must be an integer in [0, 65535]");
+            TORCH_CHECK(fcfg[19] >= 1.0 && fcfg[19] <= 65535.0 && fcfg[19] == std::floor(fcfg[19]),
+                        "fed_round_small: krum_m must be an integer in [1, 65535]");
+            p.krum_f = (int)fcfg[18]; p.krum_m = (int)fcfg[19];
+        }
         if (p.agg_rule != 0) {
             TORCH_CHECK(p.world == 1, "fed_round_small: a robust aggregation rule is single-GPU only");
             TORCH_CHECK(2 * (int64_t)p.C <= 33 * theta.size(1),
                         "fed_round_small: too many clients for the robust aggregation scratch (use fed_round_small_fits to route)");
             TORCH_CHECK(p.agg_rule != 3 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 3),
                         "fed_round_small: too many clients for the geometric-median scratch (use fed_round_small_fits to route)");
+            TORCH_CHECK(p.agg_rule != 4 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 4),
+                        "fed_round_small: too many clients for the Multi-Krum scratch (use fed_round_small_fits to route)");
         }
     }
     fdb::SmallLaunchInfo info{};
@@ -181,7 +193,7 @@ std::vector<int64_t> fed_round_small(
     return {info.cluster, info.threads, info.smem_bytes};
 }
 
-// agg_rule: 0 mean, 1 median, 2 trimmed mean, 3 geometric median (the scratch each rule needs)
+// agg_rule: 0 mean, 1 median, 2 trimmed mean, 3 geometric median, 4 Multi-Krum (the scratch each rule needs)
 bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur, bool server_opt,
                           int64_t agg_rule) {
     return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt, (int)agg_rule) != 0;
@@ -532,6 +544,69 @@ Tensor geomed_aggregate_slots(Tensor theta, Tensor cp, Tensor n, int64_t iters, 
                                                 0.999f, (float)eps, p0, p1, sp, mp, scratch.data_ptr(), cur_stream());
     TORCH_CHECK(rc != -2, "geomed_aggregate_slots: too many clients for the shared-memory staging of one column tile");
     TORCH_CHECK(rc == 0, "geomed_aggregate_slots: kernel launch failed");
+    if (sp) steps->add_((counts > 0).to(torch::kInt32));   // after the launch (same stream), as robust_aggregate_slots does
+    return counts;
+}
+
+// K21: Multi-Krum (ops/reference.py krum_aggregate_slots_: f Byzantine uploads assumed per slot, the m best-scored uploads
+// averaged, m = 1 plain Krum) of the participants (n[c, m] > 0) of every slot of cp [C, M, P] into theta [M, >= P]; dmask
+// [P] uint8 (or None) selects the entries of the distances.  The server optimizer arguments are robust_aggregate_slots'.
+// Returns the participant counts [M] (float32).
+Tensor krum_aggregate_slots(Tensor theta, Tensor cp, Tensor n, int64_t f, int64_t m, int64_t opt_kind, double lr, double momentum,
+                            double eps, c10::optional<Tensor> s0, c10::optional<Tensor> s1, c10::optional<Tensor> steps,
+                            c10::optional<Tensor> mask, c10::optional<Tensor> dmask) {
+    CHECK_CUDA_F32(theta); CHECK_CUDA_F32(cp); CHECK_CUDA_F32(n);
+    TORCH_CHECK(f >= 0 && f <= 65535, "krum_aggregate_slots: f must be in [0, 65535]");
+    TORCH_CHECK(m >= 1 && m <= 65535, "krum_aggregate_slots: m must be in [1, 65535]");
+    TORCH_CHECK(cp.is_contiguous() && cp.dim() == 3, "krum_aggregate_slots: cp must be a contiguous [C, M, P] tensor");
+    const int64_t C = cp.size(0), M = cp.size(1), P = cp.size(2);
+    TORCH_CHECK(C <= 46340 && M <= 65535, "krum_aggregate_slots: need C <= 46340 and M <= 65535");
+    TORCH_CHECK(n.device() == cp.device() && n.is_contiguous() && n.numel() == C * M,
+                "krum_aggregate_slots: n must be a contiguous float32 [C, M] tensor on the device of cp");
+    TORCH_CHECK(theta.device() == cp.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "krum_aggregate_slots: theta must be [M, >= P] with unit column stride on the device of cp");
+    const unsigned char* dp = nullptr;
+    if (dmask.has_value() && dmask->defined()) {
+        TORCH_CHECK(dmask->is_cuda() && dmask->device() == cp.device() && dmask->scalar_type() == torch::kUInt8 && dmask->is_contiguous() &&
+                    dmask->numel() == P, "krum_aggregate_slots: dmask must be a contiguous uint8 [P] tensor on the device of cp");
+        dp = dmask->data_ptr<unsigned char>();
+    }
+    float *p0 = nullptr, *p1 = nullptr;
+    int* sp = nullptr;
+    const unsigned char* mp = nullptr;
+    if (opt_kind != 0) {
+        TORCH_CHECK(opt_kind >= 1 && opt_kind <= 4, "krum_aggregate_slots: server optimizer kind must be 0..4");
+        for (const auto* t : {&s0, &s1}) {
+            if (t->has_value() && (*t)->defined()) {
+                CHECK_CUDA_F32(**t);
+                TORCH_CHECK((*t)->is_contiguous() && (*t)->dim() == 2 && (*t)->size(0) == M && (*t)->size(1) == P &&
+                            (*t)->device() == cp.device(),
+                            "krum_aggregate_slots: optimizer state must be contiguous [M, P] on the device of cp");
+            }
+        }
+        p0 = opt_ptr<float>(s0); p1 = opt_ptr<float>(s1);
+        TORCH_CHECK(p0 || (opt_kind == 1 && momentum == 0.0), "krum_aggregate_slots: this optimizer needs s0");
+        TORCH_CHECK(p1 || opt_kind == 1 || opt_kind == 3, "krum_aggregate_slots: this optimizer needs s1");
+        TORCH_CHECK(steps.has_value() && steps->defined(), "krum_aggregate_slots: a server optimizer needs the step counters");
+        CHECK_CUDA_I32(*steps);
+        TORCH_CHECK(steps->is_contiguous() && steps->numel() == M && steps->device() == cp.device(),
+                    "krum_aggregate_slots: steps must be a contiguous int32 [M] tensor on the device of cp");
+        sp = steps->data_ptr<int>();
+        if (mask.has_value() && mask->defined()) {
+            TORCH_CHECK(mask->is_cuda() && mask->device() == cp.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                        mask->numel() == P, "krum_aggregate_slots: mask must be a contiguous uint8 [P] tensor on the device of cp");
+            mp = mask->data_ptr<unsigned char>();
+        }
+    }
+    c10::cuda::CUDAGuard guard(cp.device());
+    auto counts = (n.view({C, M}) > 0).sum(0).to(torch::kFloat32);
+    const int64_t words = (fdb::krum_scratch_bytes((int)C, (int)M, P) + 7) / 8;
+    auto scratch = torch::empty({std::max<int64_t>(words, 1)}, cp.options().dtype(torch::kFloat64));
+    const int rc = fdb::krum_aggregate_launch(theta.data_ptr<float>(), theta.stride(0), cp.data_ptr<float>(), n.data_ptr<float>(),
+                                              (int)C, (int)M, P, (int)f, (int)m, dp, (int)opt_kind, (float)lr, (float)momentum, 0.9f,
+                                              0.999f, (float)eps, p0, p1, sp, mp, scratch.data_ptr(), cur_stream());
+    TORCH_CHECK(rc != -2, "krum_aggregate_slots: too many clients for the shared-memory staging");
+    TORCH_CHECK(rc == 0, "krum_aggregate_slots: kernel launch failed");
     if (sp) steps->add_((counts > 0).to(torch::kInt32));   // after the launch (same stream), as robust_aggregate_slots does
     return counts;
 }
@@ -1185,6 +1260,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("eftopk_slots", &eftopk_slots);
     m.def("robust_aggregate_slots", &robust_aggregate_slots);
     m.def("geomed_aggregate_slots", &geomed_aggregate_slots);
+    m.def("krum_aggregate_slots", &krum_aggregate_slots);
     m.def("eval_logits", &eval_logits);
     m.def("aue_sqerr", &aue_sqerr);
     m.def("ensemble_vote", &ensemble_vote);

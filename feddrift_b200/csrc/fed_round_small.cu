@@ -218,6 +218,107 @@ __device__ __noinline__ void geomed_slots(const float* slot_s, const int* pairs_
     }
 }
 
+// Multi-Krum phase (RoundParams::agg_rule == 4), after the cluster barrier that makes every CTA's published uploads visible
+// (no median columns): CTA crank takes each slot m ≡ crank (mod G) (ops/reference.py krum_aggregate_slots_) and leaves v_m
+// in its own part[m·P …] (only the slot's owner reads those entries of it).  The slot's n uploads are copied over DSMEM in
+// pair order into the CTA's gbuf.  A warp per row i computes D_ij for every j (lane per j, its P columns summed in order in
+// fp64, NaN → +∞; D_ji comes out bit-identical from row j's warp) into its distance row, ranks them, scatters the k
+// smallest to its sorted row and lane 0 sums them in order into score_i; the scores are ranked (ties to the lower row) and threads over columns
+// average the m_eff selected uploads in client order.  Scratch: per-warp distance and sorted rows [NW][C] and scores [C]
+// (double), uploads [n][P], pair list [C], selection flags [C] and n — C·(P + 4·NW + 4) + 4 floats of the NW·33·P gbuf
+// (fed_round_small_fits checks it).
+template <int P>
+__device__ __noinline__ void krum_slots(const float* slot_s, const int* pairs_s, int npairs, const float* tot_s, float* part, float* scratch,
+                                        int C, int M, int G, int crank, int warp, int NW, int lane, int f, int mkeep) {
+    cg::cluster_group cluster = cg::this_cluster();
+    const int tid = threadIdx.x, nthreads = NW * 32;
+    double* dbuf = reinterpret_cast<double*>(scratch);
+    double* sbuf = dbuf + (size_t)NW * C;
+    double* score = sbuf + (size_t)NW * C;
+    float* X = reinterpret_cast<float*>(score + C);
+    int* lst = reinterpret_cast<int*>(X + (size_t)C * P);
+    int* chosen = lst + C;
+    int* n_s = chosen + C;
+    double* dv = dbuf + (size_t)warp * C;
+    double* sv = sbuf + (size_t)warp * C;
+    for (int m = crank; m < M; m += G) {
+        if (!(tot_s[m] > 0.f)) continue;
+        if (warp == 0) {   // the slot's pairs in pair order
+            int base = 0;
+            for (int i0 = 0; i0 < npairs; i0 += 32) {
+                const int i = i0 + lane;
+                const bool on = i < npairs && pairs_s[i] % M == m;
+                const unsigned bal = __ballot_sync(0xffffffffu, on);
+                if (on) lst[base + __popc(bal & ((1u << lane) - 1u))] = i;
+                base += __popc(bal);
+            }
+            if (lane == 0) *n_s = base;
+        }
+        __syncthreads();
+        const int n = *n_s;
+        for (int idx = tid; idx < n * P; idx += nthreads) {
+            const int i = idx / P, pp = idx - i * P, pi = lst[i];
+            X[idx] = *(cluster.map_shared_rank(slot_s + (pi / G) * P + pp, pi % G));
+        }
+        for (int i = tid; i < n; i += nthreads) chosen[i] = n == 1;
+        __syncthreads();
+        const int meff = min(mkeep, n);
+        if (n > 1) {
+            const int k = min(max(n - f - 2, 1), n - 1);
+            for (int i = warp; i < n; i += NW) {
+                const float* xi = X + i * P;
+                for (int j = lane; j < n; j += 32) {
+                    if (j == i) continue;
+                    const float* xj = X + j * P;
+                    double s = 0.0;
+                    for (int pp = 0; pp < P; ++pp) {
+                        const double d = (double)__fsub_rn(xi[pp], xj[pp]);
+                        s = fma(d, d, s);
+                    }
+                    dv[j] = isnan(s) ? (double)INFINITY : s;
+                }
+                __syncwarp();
+                for (int j = lane; j < n; j += 32) {
+                    if (j == i) continue;
+                    const double a = dv[j];
+                    int rk = 0;
+                    for (int l = 0; l < n; ++l)
+                        if (l != i) rk += (dv[l] < a || (dv[l] == a && l < j)) ? 1 : 0;
+                    if (rk < k) sv[rk] = a;
+                }
+                __syncwarp();
+                if (lane == 0) {
+                    double s = 0.0;
+                    for (int r = 0; r < k; ++r) s += sv[r];
+                    score[i] = s;
+                }
+                __syncwarp();
+            }
+            __syncthreads();
+            for (int i = tid; i < n; i += nthreads) {
+                const double a = score[i];
+                int rk = 0;
+                for (int l = 0; l < n; ++l) rk += (score[l] < a || (score[l] == a && l < i)) ? 1 : 0;
+                chosen[i] = rk < meff;
+            }
+            __syncthreads();
+        }
+        float* v = part + m * P;
+        for (int pp = tid; pp < P; pp += nthreads) {
+            float acc = 0.f;
+            bool first = true;
+            for (int i = 0; i < n; ++i)
+                if (chosen[i]) {
+                    const float x = X[i * P + pp];
+                    acc = first ? x : __fadd_rn(acc, x);
+                    first = false;
+                }
+            v[pp] = meff > 1 ? __fdiv_rn(acc, (float)meff) : acc;
+        }
+        __syncthreads();   // the next slot rewrites the scratch
+    }
+}
+
 // sample coordinates of element i of the current mini-batch
 struct BatchSel {
     int mode;        // 0/1: contiguous [lo, lo+n) of (tb, c);  2: list
@@ -231,7 +332,7 @@ constexpr int kCompNone = 0, kCompQsgd = 1, kCompEfTopk = 2;
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
 // its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kComp: the upload compression
 // (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0) and kRobust: a median / trimmed-mean aggregation rule
-// or geometric median (p.agg_rule != 0), separate for the same reason
+// or geometric median or Multi-Krum (p.agg_rule != 0), separate for the same reason
 template <class Net, bool kDefend, bool kProx, int kComp, bool kRobust>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
@@ -693,12 +794,17 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                 // columns e ≡ crank (mod G) into its part_s, one warp per column over DSMEM (pair i of the compacted list
                 // lives in CTA i mod G, slot i / G; pairs_s is the same in every CTA), with the warp's gbuf as scratch
                 if (G > 1) cluster.sync(); else __syncthreads();
-                robust_columns<P>(slot_s, pairs_s, npairs, tot_s, theta_s, part_s + buf * MP, smem + L.gbuf + warp * (P * 33),
-                                  M, G, crank, warp, NW, lane, p.agg_rule != 2, p.trim_ratio);
-                if (p.agg_rule == 3) {   // geometric median: start from that median, CTA k refines the slots m ≡ k (mod G)
-                    if (G > 1) cluster.sync(); else __syncthreads();
-                    geomed_slots<P>(slot_s, pairs_s, npairs, tot_s, part_s + buf * MP, smem + L.gbuf, C, M, G, crank, warp, NW, lane,
-                                    p.gm_iters, p.gm_nu);
+                if (p.agg_rule == 4) {   // Multi-Krum needs no median: CTA k selects and averages the slots m ≡ k (mod G)
+                    krum_slots<P>(slot_s, pairs_s, npairs, tot_s, part_s + buf * MP, smem + L.gbuf, C, M, G, crank, warp, NW, lane,
+                                  p.krum_f, p.krum_m);
+                } else {
+                    robust_columns<P>(slot_s, pairs_s, npairs, tot_s, theta_s, part_s + buf * MP, smem + L.gbuf + warp * (P * 33),
+                                      M, G, crank, warp, NW, lane, p.agg_rule != 2, p.trim_ratio);
+                    if (p.agg_rule == 3) {   // geometric median: start from that median, CTA k refines the slots m ≡ k (mod G)
+                        if (G > 1) cluster.sync(); else __syncthreads();
+                        geomed_slots<P>(slot_s, pairs_s, npairs, tot_s, part_s + buf * MP, smem + L.gbuf, C, M, G, crank, warp, NW,
+                                        lane, p.gm_iters, p.gm_nu);
+                    }
                 }
             }
             if (G > 1) cluster.sync(); else __syncthreads();
@@ -707,8 +813,8 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     const int m = e / P;
                     if (tot_s[m] > 0.f) {
                         float v = 0.f;
-                        if constexpr (kRobust)   // the column's owner (geometric median: the slot's owner)
-                            v = *(cluster.map_shared_rank(part_s + buf * MP + e, p.agg_rule == 3 ? m % G : e % G));
+                        if constexpr (kRobust)   // the column's owner (geometric median, Multi-Krum: the slot's owner)
+                            v = *(cluster.map_shared_rank(part_s + buf * MP + e, p.agg_rule >= 3 ? m % G : e % G));
                         else for (int rk = 0; rk < G; ++rk) v += *(cluster.map_shared_rank(part_s + buf * MP + e, rk));
                         if (p.sopt_kind) {
                             const float ts = (float)(sstep_s[m] + 1);
@@ -1032,15 +1138,18 @@ static int fits_round(int C, int M, bool server_opt) {
 }
 
 // 1 when the fused kernel can run this federation: instantiated shape, t_cur < kTmax, shared-memory layout (with the server
-// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule (agg_rule 1..3) 2·C ≤ 33·P (a slot's
+// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule (agg_rule 1..4) 2·C ≤ 33·P (a slot's
 // uploads and their ranked copy fit the ranking warp's gbuf); the geometric median (3) also needs C·(P + 2) + 4 ≤ the
-// CTA's gbuf (a slot's uploads, weights and pair list)
+// CTA's gbuf (a slot's uploads, weights and pair list), Multi-Krum (4) C·(P + 4·warps + 4) + 4 ≤ it (a slot's uploads,
+// per-warp fp64 distance and sorted rows, fp64 scores, pair list and selection flags)
 int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule) {
     if (t_cur >= kTmax) return 0;
 #define FDB_CASE(K, I, H, O)                                                                                            \
     if (kind == K && din == I && (K == 0 || hid == H) && dout == O)                                                     \
         return fits_round<Mlp<K, I, H, O>>(C, M, server_opt) && (agg_rule == 0 || 2 * C <= 33 * Mlp<K, I, H, O>::P) && \
                (agg_rule != 3 || (long long)C * (Mlp<K, I, H, O>::P + 2) + 4 <=                                          \
+                                     (long long)SmallCfg<Mlp<K, I, H, O>>::kWarps * 33 * Mlp<K, I, H, O>::P) &&          \
+               (agg_rule != 4 || (long long)C * (Mlp<K, I, H, O>::P + 4 * SmallCfg<Mlp<K, I, H, O>>::kWarps + 4) + 4 <= \
                                      (long long)SmallCfg<Mlp<K, I, H, O>>::kWarps * 33 * Mlp<K, I, H, O>::P);
     FDB_MLP_SHAPES(FDB_CASE)
 #undef FDB_CASE

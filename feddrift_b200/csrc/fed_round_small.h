@@ -57,6 +57,9 @@ struct RoundParams {
     // coordinate-wise median, weights 1 / max(gm_nu, distance)
     int gm_iters;
     double gm_nu;
+    // agg_rule 4: Multi-Krum (ops/reference.py krum_aggregate_slots_): the average of the min(krum_m, n) uploads whose
+    // summed squared distances to their clamp(n − krum_f − 2, 1, n − 1) nearest neighbours are smallest
+    int krum_f, krum_m;
     float* client_out; // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs

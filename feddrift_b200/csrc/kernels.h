@@ -43,6 +43,14 @@ int geomed_aggregate_launch(float* theta, long long t_stride, const float* cp, c
                             double nu, const unsigned char* dmask, int opt_kind, float lr, float momentum, float b1, float b2,
                             float eps, float* s0, float* s1, const int* steps, const unsigned char* mask, void* scratch,
                             cudaStream_t stream);
+// robust_agg.cu (K21): Multi-Krum (f assumed Byzantine uploads per slot, the mkeep best-scored uploads averaged; dmask [P]
+// uint8 or null: the entries in the distances) of the same participants into theta, server step as K19.  scratch holds
+// krum_scratch_bytes(C, M, P) bytes (8-byte aligned).  -2: C too large for the shared-memory staging
+long long krum_scratch_bytes(int C, int M, long long P);
+int krum_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, int C, int M, long long P, int f,
+                          int mkeep, const unsigned char* dmask, int opt_kind, float lr, float momentum, float b1, float b2,
+                          float eps, float* s0, float* s1, const int* steps, const unsigned char* mask, void* scratch,
+                          cudaStream_t stream);
 // aggregate_peer.cu : multi-GPU reduce-scatter + apply + all-gather over NVLink peer memory (cooperative launch)
 int fedavg_reduce_apply_peer_launch(const float* cp, const int* cidx, const float* n, int C, int M, int P, int theta_stride, int world, int rank,
                                     const long long* part_ptrs, const long long* theta_ptrs, const long long* tot_ptrs,

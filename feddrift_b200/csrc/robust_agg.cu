@@ -26,6 +26,18 @@
 //                 order), and marks the slot kept (n ≤ 2 or W = 0) or NaN (a NaN distance);
 //   pass R + 1    v^R into θ_m through the store phase (server step included).
 // No float atomics and a grid that depends only on the device and the shape, so every launch gives the same bits.
+//
+// K21: Multi-Krum (ops/reference.py krum_aggregate_slots_ is the definition) of the same participants, in three launches:
+//   distance pass  K19's compaction and tile staging; thread per pair (i < j), the fp64 partial Σ fl32(x_i − x_j)² over
+//                  the tile's trainable columns, added in tile order into the pair's accumulator (shared memory when the
+//                  n(n − 1)/2 pairs fit beside a tile of ≥ 32 columns, else the CTA's own row in global memory, so any C
+//                  the staging takes works); stored per CTA to [M, gridX, npairs];
+//   select step    one CTA per slot sums the partials in CTA order, warp per row ranks its distances and sums the k
+//                  smallest in order into the score, ranks the scores and writes the m_eff selected rows (client order);
+//   store pass     the fp32 sum of the selected rows in client order, one division by m_eff, into θ_m through the store
+//                  phase (server step included).
+// The participants' rows are read once (the store pass reads the m_eff selected ones again).  No float atomics and a grid
+// fixed by the device and the shape, so every launch gives the same bits.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -317,6 +329,183 @@ __global__ void __launch_bounds__(kThreads) geomed_finish_kernel(const float* __
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------- K21
+constexpr long long kKrumPartBudget = 1LL << 23;   // doubles of [M, gridX, npairs] partials (64 MB) the grid may use
+
+__host__ __device__ inline long long krum_npairs(int C) { return C >= 2 ? (long long)C * (C - 1) / 2 : 1; }
+
+// bytes of dynamic shared memory of krum_dist_kernel: the pair accumulators [npairs(C)] (double; only when they stay on
+// chip), tile [C][T + 1], participant list [C], the tile's distance mask [T] (bytes)
+inline size_t krum_dist_smem_bytes(int C, int T, bool acc_on_chip) {
+    return (acc_on_chip ? (size_t)krum_npairs(C) * sizeof(double) : 0) + (size_t)C * (T + 2) * sizeof(float) + T + 16;
+}
+
+// bytes of dynamic shared memory of krum_select_kernel: scores [C] and two distance rows [C] per warp (double), the
+// participant list and the selection flags [C] (int)
+inline size_t krum_select_smem_bytes(int C) { return (size_t)C * (1 + 2 * kWarps) * sizeof(double) + (size_t)C * 8 + 16; }
+
+// pair p of the lower triangle, p = j(j − 1)/2 + i with 0 ≤ i < j (consecutive p: consecutive rows i of one j)
+__device__ __forceinline__ void krum_pair(int p, int* i, int* j) {
+    int r = (int)((1.0 + sqrt(1.0 + 8.0 * (double)p)) * 0.5);
+    while ((long long)r * (r - 1) / 2 > p) --r;
+    while ((long long)(r + 1) * r / 2 <= p) ++r;
+    *j = r;
+    *i = p - (int)((long long)r * (r - 1) / 2);
+}
+
+// Distance pass (grid (gridX, M), persistent over the column tiles of each slot like K19): the fp64 partials
+// Σ fl32(x_i − x_j)² over this CTA's trainable columns of every pair of participants, thread per pair, each tile's sum
+// added in tile order into the pair's accumulator (on chip when they fit, else the CTA's own row of part), stored to
+// part [M, gridX, npairs(C)].  The participants' rows are read once.
+__global__ void __launch_bounds__(kThreads) krum_dist_kernel(const float* __restrict__ cp, const float* __restrict__ n, int C,
+                                                            int M, long long P, int T, bool acc_on_chip,
+                                                            const unsigned char* __restrict__ dmask, double* __restrict__ part) {
+    extern __shared__ __align__(16) float sm[];
+    const long long npmax = krum_npairs(C);
+    double* dacc = reinterpret_cast<double*>(sm);
+    float* tile = reinterpret_cast<float*>(dacc + (acc_on_chip ? npmax : 0));   // [nrows][T + 1]
+    int* rows = reinterpret_cast<int*>(tile + (size_t)C * (T + 1));
+    unsigned char* mk = reinterpret_cast<unsigned char*>(rows + C);          // [T]
+    __shared__ int cnt_s;
+    const int tid = threadIdx.x;
+    const int m = blockIdx.y;
+    const int cnt = compact_participants(n, C, M, m, rows, &cnt_s);
+    if (cnt < 2) return;
+    const int np = cnt * (cnt - 1) / 2;
+    double* mine = part + ((size_t)m * gridDim.x + blockIdx.x) * npmax;
+    double* acc = acc_on_chip ? dacc : mine;
+    for (int p = tid; p < np; p += kThreads) acc[p] = 0.0;
+    const size_t rstride = (size_t)M * P;
+    const int pitch = T + 1;
+    const bool vec = ((P & 3) == 0) && ((((uintptr_t)cp) & 15) == 0);
+    const long long ntiles = (P + T - 1) / T;
+    for (long long tile_i = blockIdx.x; tile_i < ntiles; tile_i += gridDim.x) {
+        const long long col0 = tile_i * T;
+        const int tw = (int)min((long long)T, P - col0);
+        stage_tile(tile, cp, rows, cnt, rstride, m, P, col0, T, tw, vec);
+        for (int j = tid; j < tw; j += kThreads) mk[j] = dmask ? dmask[col0 + j] : 1;
+        __syncthreads();
+        for (int p = tid; p < np; p += kThreads) {
+            int i, j;
+            krum_pair(p, &i, &j);
+            const float* a = tile + (size_t)i * pitch;
+            const float* b = tile + (size_t)j * pitch;
+            double s = 0.0;
+            for (int c = 0; c < tw; ++c)
+                if (mk[c]) {
+                    const double d = (double)__fsub_rn(a[c], b[c]);
+                    s = fma(d, d, s);
+                }
+            acc[p] += s;
+        }
+        __syncthreads();   // the next tile overwrites tile / mk
+    }
+    if (acc_on_chip)
+        for (int p = tid; p < np; p += kThreads) mine[p] = dacc[p];
+}
+
+// Select step, one CTA per slot: D_ij = the CTA partials summed in CTA order (NaN → +∞, written over the first CTA's
+// partial), score_i = Σ of the k = clamp(n − f − 2, 1, n − 1) smallest D_ij (j ≠ i) in ascending order, ties by j (warp
+// per row: rank, scatter, lane 0 sums), then the m_eff = min(mkeep, n) best scores (ties to the lower row) as client
+// indices in client order into sel [M, C] and m_eff into selcnt [M] (n = 1: that row; n = 0: 0).
+__global__ void __launch_bounds__(kThreads) krum_select_kernel(const float* __restrict__ n, int C, int M, int gx, int f, int mkeep,
+                                                              double* __restrict__ part, int* __restrict__ sel,
+                                                              int* __restrict__ selcnt) {
+    extern __shared__ __align__(16) float sm[];
+    double* score = reinterpret_cast<double*>(sm);            // [C]
+    double* dbuf = score + C;                                 // [kWarps][C] distances of the warp's row
+    double* sbuf = dbuf + (size_t)kWarps * C;                 // [kWarps][C] the same, sorted
+    int* rows = reinterpret_cast<int*>(sbuf + (size_t)kWarps * C);
+    int* chosen = rows + C;
+    __shared__ int cnt_s;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int m = blockIdx.x;
+    const int cnt = compact_participants(n, C, M, m, rows, &cnt_s);
+    if (cnt < 2) {
+        if (tid == 0) {
+            if (cnt == 1) sel[(size_t)m * C] = rows[0];
+            selcnt[m] = cnt;
+        }
+        return;
+    }
+    const long long npmax = krum_npairs(C);
+    const int np = cnt * (cnt - 1) / 2;
+    double* D = part + (size_t)m * gx * npmax;
+    for (int p = tid; p < np; p += kThreads) {
+        double d = 0.0;
+        for (int b = 0; b < gx; ++b) d += D[(size_t)b * npmax + p];
+        D[p] = isnan(d) ? (double)INFINITY : d;
+    }
+    __syncthreads();
+    const int k = min(max(cnt - f - 2, 1), cnt - 1);
+    double* dv = dbuf + (size_t)warp * C;
+    double* sv = sbuf + (size_t)warp * C;
+    for (int i = warp; i < cnt; i += kWarps) {
+        for (int j = lane; j < cnt; j += 32)
+            if (j != i) dv[j] = D[j > i ? j * (j - 1) / 2 + i : i * (i - 1) / 2 + j];
+        __syncwarp();
+        for (int j = lane; j < cnt; j += 32) {
+            if (j == i) continue;
+            const double a = dv[j];
+            int rk = 0;
+            for (int l = 0; l < cnt; ++l) {
+                if (l == i) continue;
+                const double x = dv[l];
+                rk += (x < a || (x == a && l < j)) ? 1 : 0;
+            }
+            if (rk < k) sv[rk] = a;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            double s = 0.0;
+            for (int r = 0; r < k; ++r) s += sv[r];
+            score[i] = s;
+        }
+        __syncwarp();
+    }
+    __syncthreads();
+    const int meff = min(mkeep, cnt);
+    for (int i = tid; i < cnt; i += kThreads) {
+        const double a = score[i];
+        int rk = 0;
+        for (int l = 0; l < cnt; ++l) rk += (score[l] < a || (score[l] == a && l < i)) ? 1 : 0;
+        chosen[i] = rk < meff;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int q = 0;
+        for (int i = 0; i < cnt; ++i)
+            if (chosen[i]) sel[(size_t)m * C + q++] = rows[i];
+        selcnt[m] = q;
+    }
+}
+
+// Store pass (grid (gridX, M)): v_e = the fp32 sum of the selected rows in client order from the first one, one division
+// by m_eff when m_eff > 1, into θ_m through K19's store phase (server step included).  Reads only the selected rows.
+__global__ void __launch_bounds__(kThreads) krum_store_kernel(float* __restrict__ theta, long long t_stride,
+                                                             const float* __restrict__ cp, int C, int M, long long P,
+                                                             const int* __restrict__ sel, const int* __restrict__ selcnt,
+                                                             RobustOpt so) {
+    extern __shared__ __align__(16) float sm[];
+    int* rows = reinterpret_cast<int*>(sm);
+    const int m = blockIdx.y;
+    const int q = selcnt[m];
+    if (q == 0) return;
+    for (int i = threadIdx.x; i < q; i += kThreads) rows[i] = sel[(size_t)m * C + i];
+    __syncthreads();
+    float bc1, bc2;
+    server_bias_corrections(so, m, &bc1, &bc2);
+    const size_t rstride = (size_t)M * P;
+    const float* base = cp + (size_t)m * P;
+    float* out = theta + (size_t)m * t_stride;
+    for (long long e = (long long)blockIdx.x * kThreads + threadIdx.x; e < P; e += (long long)gridDim.x * kThreads) {
+        float v = __ldcs(base + (size_t)rows[0] * rstride + e);
+        for (int i = 1; i < q; ++i) v = __fadd_rn(v, __ldcs(base + (size_t)rows[i] * rstride + e));
+        if (q > 1) v = __fdiv_rn(v, (float)q);
+        store_entry(out, e, v, so, (size_t)m, P, bc1, bc2);
+    }
+}
+
 }  // namespace
 
 int robust_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, int C, int M, long long P,
@@ -393,6 +582,62 @@ int geomed_aggregate_launch(float* theta, long long t_stride, const float* cp, c
         if (cudaGetLastError() != cudaSuccess) return -4;
     }
     return 0;
+}
+
+namespace {
+// K21's distance tile: the widest tile of at least 32 columns with the pair accumulators on chip, else the widest tile
+// with them in the CTA's row of the partials
+struct KrumPlan {
+    int T;
+    bool acc_on_chip;
+};
+inline KrumPlan krum_plan(int C) {
+    for (int T = 128; T >= 32; T >>= 1)
+        if (krum_dist_smem_bytes(C, T, true) <= (size_t)kSmemBudget) return {T, true};
+    return {tile_width(C, [](int c, int t) { return (krum_dist_smem_bytes(c, t, false) + 3) / 4; }), false};
+}
+
+inline int krum_grid_x(int C, int M, long long P) {
+    const KrumPlan kp = krum_plan(C);
+    const long long cap = max(1LL, kKrumPartBudget / ((long long)M * krum_npairs(C)));
+    return (int)min((long long)persistent_grid_x((P + kp.T - 1) / kp.T, M), cap);
+}
+}  // namespace
+
+long long krum_scratch_bytes(int C, int M, long long P) {
+    if (C <= 0 || M <= 0 || P <= 0) return 0;
+    return (long long)M * krum_grid_x(C, M, P) * krum_npairs(C) * 8 + (long long)M * C * 4 + (long long)M * 4;
+}
+
+int krum_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, int C, int M, long long P, int f,
+                          int mkeep, const unsigned char* dmask, int opt_kind, float lr, float momentum, float b1, float b2,
+                          float eps, float* s0, float* s1, const int* steps, const unsigned char* mask, void* scratch,
+                          cudaStream_t stream) {
+    if (C <= 0 || M <= 0 || P <= 0) return 0;
+    if (M > 65535) return -5;
+    const KrumPlan kp = krum_plan(C);
+    const size_t dsmem = krum_dist_smem_bytes(C, kp.T, kp.acc_on_chip), ssmem = krum_select_smem_bytes(C);
+    if (dsmem > 227 * 1024 || ssmem > 227 * 1024) return -2;
+    if (dsmem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute(krum_dist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dsmem);
+        if (e != cudaSuccess) return -3;
+    }
+    if (ssmem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute(krum_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem);
+        if (e != cudaSuccess) return -3;
+    }
+    const int gx = krum_grid_x(C, M, P);
+    char* sp = static_cast<char*>(scratch);
+    double* part = reinterpret_cast<double*>(sp);         sp += (size_t)M * gx * krum_npairs(C) * 8;
+    int* sel = reinterpret_cast<int*>(sp);                sp += (size_t)M * C * 4;
+    int* selcnt = reinterpret_cast<int*>(sp);
+    krum_dist_kernel<<<dim3((unsigned)gx, (unsigned)M), kThreads, dsmem, stream>>>(cp, n, C, M, P, kp.T, kp.acc_on_chip, dmask,
+                                                                                    part);
+    krum_select_kernel<<<M, kThreads, ssmem, stream>>>(n, C, M, gx, f, mkeep, part, sel, selcnt);
+    const RobustOpt so{opt_kind, lr, momentum, b1, b2, eps, s0, s1, steps, mask};
+    const dim3 sgrid((unsigned)persistent_grid_x((P + kThreads - 1) / kThreads, M), (unsigned)M);
+    krum_store_kernel<<<sgrid, kThreads, (size_t)C * sizeof(int), stream>>>(theta, t_stride, cp, C, M, P, sel, selcnt, so);
+    return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 
 }  // namespace fdb

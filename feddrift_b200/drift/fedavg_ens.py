@@ -34,8 +34,8 @@ from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, compress_seed, compression_params, geomed_params, prox_mu_param, topk_k,
-                             topk_ratio_param)
+from ..ops.reference import (aggregation_params, compress_seed, compression_params, geomed_params, krum_params,
+                             prox_mu_param, topk_k, topk_ratio_param)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
@@ -425,7 +425,16 @@ class _BaseAggregator:
         # the geometric median (--geomed_iters / --geomed_nu, validated whatever the rule) carries (rule, β, R, ν); its
         # distances cover the trainable entries (defense_mask)
         gm_iters, gm_nu = geomed_params(getattr(args, "geomed_iters", 4), getattr(args, "geomed_nu", 1e-6))
-        self.agg_rule = None if rule == "mean" else ((rule, beta, gm_iters, gm_nu) if rule == "geometric_median" else (rule, beta))
+        # Multi-Krum (--krum_f / --krum_m, validated whatever the rule) carries (rule, β, f, m), distances as above
+        krum_f, krum_m = krum_params(getattr(args, "krum_f", 1), getattr(args, "krum_m", 1))
+        if rule == "mean":
+            self.agg_rule = None
+        elif rule == "geometric_median":
+            self.agg_rule = (rule, beta, gm_iters, gm_nu)
+        elif rule == "multi_krum":
+            self.agg_rule = (rule, beta, krum_f, krum_m)
+        else:
+            self.agg_rule = (rule, beta)
         # upload compression (--compression qsgd): each arriving upload is quantized against bank.theta[m]; its draws follow
         # this aggregator's round counter, advanced when a round's uploads are complete (packages without the flags: none)
         self.q_level, self.q_bucket = compression_params(getattr(args, "compression", "none") or "none",
@@ -503,7 +512,7 @@ class _BaseAggregator:
             a = self.args
             seed = int(getattr(a, "dummy_arg", 0)) * 7919 + 13 + 1000003 * int(getattr(a, "curr_train_iteration", 0) or 0)
             self.defense.defend_slots_(self.upload, self.bank.theta, n, self.defense_mask, seed, self._defense_round)
-        if self.agg_rule is not None and self.agg_rule[0] == "geometric_median":
+        if self.agg_rule is not None and self.agg_rule[0] in ("geometric_median", "multi_krum"):
             ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt, self.agg_rule, mask=self.defense_mask)
         else:
             ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt, self.agg_rule)

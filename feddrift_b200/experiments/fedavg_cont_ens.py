@@ -68,11 +68,15 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--topk_ratio", type=float, default=0.01, help="eftopk: fraction ρ of the trainable entries kept, 0 < ρ <= 1")
     # Byzantine-robust cluster aggregation (Yin et al., 2018): the coordinate-wise median or β-trimmed mean of the slot's
     # uploads (after compression and the defense), each participant counted once, instead of the weighted average
-    a("--aggregation_rule", type=str, default="mean", choices=["mean", "median", "trimmed_mean", "geometric_median"])
+    a("--aggregation_rule", type=str, default="mean", choices=["mean", "median", "trimmed_mean", "geometric_median", "multi_krum"])
     a("--trim_ratio", type=float, default=0.1, help="trimmed_mean: fraction β dropped at each end, 0 <= β < 0.5")
     # geometric median (RFA, Pillutla et al.): smoothed Weiszfeld steps from the coordinate-wise median
     a("--geomed_iters", type=int, default=4, help="geometric_median: Weiszfeld iterations R, 1..100")
     a("--geomed_nu", type=float, default=1e-6, help="geometric_median: smoothing ν > 0 (weights 1 / max(ν, distance))")
+    # Multi-Krum (Blanchard et al., 2017): the average of the m uploads closest to their n − f − 2 nearest neighbours; one
+    # rule with one name, --krum_m 1 is plain Krum
+    a("--krum_f", type=int, default=1, help="multi_krum: Byzantine uploads f assumed per slot, 0..65535")
+    a("--krum_m", type=int, default=1, help="multi_krum: uploads m averaged, 1..65535 (1: Krum)")
     # FedProx local training: every client step minimises CE + mu/2‖w − w_m‖², w_m the cluster model it received (0 = off)
     a("--fedprox_mu", type=float, default=0.0)
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)

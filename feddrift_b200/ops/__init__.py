@@ -21,6 +21,7 @@ Kernel map (SURVEY §2.9 numbering):
   K18 eftopk_slots_ (top-k + error feedback)      csrc/sparsify.cu
   K19 robust_aggregate_slots_ (median / trimmed mean)   csrc/robust_agg.cu
   K20 geomed_aggregate_slots_ (geometric median)        csrc/robust_agg.cu
+  K21 krum_aggregate_slots_ (Multi-Krum)                csrc/robust_agg.cu
 """
 from __future__ import annotations
 
@@ -58,9 +59,12 @@ def cluster_aggregate_(theta, client_params, n, server_opt=None, rule=None, mask
     ``rule`` = ``(aggregation_rule, trim_ratio)`` with rule 'median' or 'trimmed_mean' replaces the weighted mean by K19
     (``robust_aggregate_slots_``: the participants n > 0 count once each) and returns the participant counts [M]; None or
     'mean' is the weighted mean above.  ``rule`` = ``('geometric_median', trim_ratio, iters, nu)`` takes K20
-    (``geomed_aggregate_slots_``) instead, with ``mask`` the trainable entries its distances cover (None: all)."""
+    (``geomed_aggregate_slots_``) instead, with ``mask`` the trainable entries its distances cover (None: all), and
+    ``('multi_krum', trim_ratio, f, m)`` takes K21 (``krum_aggregate_slots_``) with the same ``mask``."""
     if rule is not None and rule[0] == "geometric_median":
         return geomed_aggregate_slots_(theta, client_params, n, rule[2], rule[3], server_opt, mask)
+    if rule is not None and rule[0] == "multi_krum":
+        return krum_aggregate_slots_(theta, client_params, n, rule[2], rule[3], server_opt, mask)
     if rule is not None and rule[0] != "mean":
         return robust_aggregate_slots_(theta, client_params, n, rule[0], rule[1], server_opt)
     if server_opt is not None:
@@ -118,6 +122,32 @@ def geomed_aggregate_slots_(theta, uploads, n, iters: int = 4, nu: float = 1e-6,
         return ref.geomed_aggregate_slots_(theta, uploads, n, iters, nu, mask)
     avg = theta.clone()
     counts = ref.geomed_aggregate_slots_(avg, uploads, n, iters, nu, mask)
+    so = server_opt
+    ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
+    return counts
+
+
+def krum_aggregate_slots_(theta, uploads, n, f: int = 1, m: int = 1, server_opt=None, mask=None):
+    """K21: θ_s ← Multi-Krum of the uploads ``uploads[c, s]`` with ``n[c, s] > 0`` (each counted once) for every slot with
+    a participant: the average of the min(``m``, n) uploads whose summed squared distances to their clamp(n − ``f`` − 2, 1,
+    n − 1) nearest neighbours are smallest (``m`` = 1: plain Krum, the slot becomes one upload); ``theta`` may be a padded
+    bank; ``mask`` [P] (bool, None = all) selects the entries of the distances (BatchNorm statistics are averaged but left
+    out).  ``server_opt`` then steps each such slot on θ_s − v and advances its counter.  See
+    ``reference.krum_aggregate_slots_``; returns the participant counts [M]."""
+    f, m = ref.krum_params(f, m)
+    if native(theta, uploads):
+        nn = n.float().contiguous()
+        dm = None if mask is None else mask.reshape(-1)[: uploads.shape[2]].to(uploads.device, torch.uint8).contiguous()
+        if server_opt is None:
+            return _ext.load().krum_aggregate_slots(theta, uploads.contiguous(), nn, f, m, 0, 0.0, 0.0, 1e-8,
+                                                    None, None, None, None, dm)
+        so = server_opt
+        return _ext.load().krum_aggregate_slots(theta, uploads.contiguous(), nn, f, m, so.kind, so.lr, so.momentum, so.eps,
+                                                so.s0, so.s1, so.step, so._mask_u8, dm)
+    if server_opt is None:
+        return ref.krum_aggregate_slots_(theta, uploads, n, f, m, mask)
+    avg = theta.clone()
+    counts = ref.krum_aggregate_slots_(avg, uploads, n, f, m, mask)
     so = server_opt
     ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
     return counts

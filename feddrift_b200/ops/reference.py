@@ -226,6 +226,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     ignored) instead of the weighted average; the server optimizer then steps on θ_m − that statistic.
     ``aggregation_rule`` 'geometric_median' with ``geomed_iters`` R (4) and ``geomed_nu`` ν (1e-6), validated whatever the
     rule by ``geomed_params``: the same, with ``geomed_aggregate_slots_`` (every entry is trainable in these MLPs).
+    ``aggregation_rule`` 'multi_krum' with ``krum_f`` f (1) and ``krum_m`` m (1), validated whatever the rule by
+    ``krum_params``: the same, with ``krum_aggregate_slots_``.
     ``fedprox_mu`` (absent or 0: off): every local
     step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
     (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
@@ -262,6 +264,7 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
         st["ef_residual"] = torch.zeros(C, M, P, dtype=torch.float32)
     agg_rule, trim_ratio = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
     gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
+    krum_f, krum_m = krum_params(st.get("krum_f", 1), st.get("krum_m", 1))
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -337,6 +340,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                 up[c, m], trained[c, m] = p, 1.0
             if agg_rule == "geometric_median":
                 geomed_aggregate_slots_(avg, up, trained, gm_iters, gm_nu)
+            elif agg_rule == "multi_krum":
+                krum_aggregate_slots_(avg, up, trained, krum_f, krum_m)
             else:
                 robust_aggregate_slots_(avg, up, trained, agg_rule, trim_ratio)
         for m in range(M):
@@ -697,13 +702,14 @@ def topk_upload_bits(P_train: int, P_other: int, k: int) -> int:
     return k * (32 + max(P - 1, 0).bit_length()) + 32 * P_other
 
 
-AGGREGATION_RULES = ("mean", "median", "trimmed_mean", "geometric_median")
+# Multi-Krum has one name: ``multi_krum`` with ``krum_m`` = 1 is plain Krum, and a bare ``krum`` is an unknown rule.
+AGGREGATION_RULES = ("mean", "median", "trimmed_mean", "geometric_median", "multi_krum")
 
 
 def aggregation_params(rule, trim_ratio) -> Tuple[str, float]:
     """Validated ``(--aggregation_rule, --trim_ratio)``.  The rule is one of ``mean`` (weighted FedAvg), ``median``,
-    ``trimmed_mean`` or ``geometric_median``; β is checked whatever the rule and must be a finite number with 0 ≤ β < 0.5.
-    Raises ``ValueError``."""
+    ``trimmed_mean``, ``geometric_median`` or ``multi_krum``; β is checked whatever the rule and must be a finite number
+    with 0 ≤ β < 0.5.  Raises ``ValueError``."""
     rule = "mean" if rule is None else rule
     if rule not in AGGREGATION_RULES:
         raise ValueError(f"aggregation_rule must be one of {', '.join(AGGREGATION_RULES)} (got {rule!r})")
@@ -851,6 +857,99 @@ def geomed_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch
             v = new
         theta[m, :P] = v.to(theta.device)
     return counts
+
+
+KRUM_MAX = 65535
+
+
+def krum_params(f, m) -> Tuple[int, int]:
+    """Validated ``(--krum_f, --krum_m)``, checked whatever the rule: f an int with 0 ≤ f ≤ 65535 (the Byzantine uploads a
+    slot is assumed to hold), m an int with 1 ≤ m ≤ 65535 (the uploads kept; 1 is plain Krum).  A bool is not an int here.
+    Raises ``ValueError``."""
+    if isinstance(f, bool) or not isinstance(f, (int, np.integer)) or not 0 <= int(f) <= KRUM_MAX:
+        raise ValueError(f"krum_f must be an int in [0, {KRUM_MAX}] (got {f!r})")
+    if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 1 <= int(m) <= KRUM_MAX:
+        raise ValueError(f"krum_m must be an int in [1, {KRUM_MAX}] (got {m!r})")
+    return int(f), int(m)
+
+
+def krum_neighbours(n: int, f: int) -> int:
+    """Neighbours a Krum score sums over in a slot of n ≥ 2 uploads: clamp(n − f − 2, 1, n − 1).  Cluster sizes vary, so
+    f is a per-slot assumption and every n is valid (f need not satisfy n ≥ 2f + 3)."""
+    return min(max(n - f - 2, 1), n - 1)
+
+
+def krum_select(D, f: int, m: int) -> Tuple[list, list]:
+    """Krum scores and selection from the n × n distances ``D`` (nested lists of floats, n ≥ 2, +∞ for NaN): score_i is
+    the float64 sum, from 0 in ascending order with ties by j, of the ``krum_neighbours(n, f)`` smallest D_ij over j ≠ i;
+    the selection is the min(m, n) rows of smallest score (ties to the lower row, +∞ last), in ascending row order."""
+    k = len(D)
+    nb = krum_neighbours(k, f)
+    scores = []
+    for i in range(k):
+        sc = 0.0
+        for d, _ in sorted((D[i][j], j) for j in range(k) if j != i)[:nb]:
+            sc += d
+        scores.append(sc)
+    return scores, sorted(sorted(range(k), key=lambda i: (scores[i], i))[:min(m, k)])
+
+
+def krum_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch.Tensor, f: int = 1, m: int = 1,
+                          mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Multi-Krum (K21; Blanchard et al., NeurIPS 2017), in place.  For every slot the participants x_1…x_n are the rows c
+    with ``n[c, slot] > 0`` in ascending c, each counted once (the weights are ignored, as in ``robust_aggregate_slots_``);
+    ``theta`` may be a padded bank.
+
+    * n = 1: v is that upload.
+    * Distances (n ≥ 2): D_ij = Σ_e mask_e · (double) fl32(x_ie − x_je)², the fp32 difference squared and summed in
+      float64 over the trainable entries (``mask``, None = all, so BatchNorm statistics stay out); D_ij = D_ji, and a NaN
+      distance counts as +∞.
+    * Scores: with k = ``krum_neighbours(n, f)``, score_i is the float64 sum, from 0 in ascending order (ties by j), of the
+      k smallest D_ij over j ≠ i.
+    * Selection: the m_eff = min(m, n) rows of smallest score; ties go to the lower client index, +∞ ranks last.
+    * Result: v_e = the fp32 sum of x_ie over the selected rows in client order, starting from the first selected value,
+      then one round-to-nearest division by m_eff (none when m_eff = 1, so the slot becomes that upload bit for bit), for
+      every entry (BatchNorm statistics included).
+
+    A NaN or ±∞ row has only infinite distances, so it is never selected while enough finite rows remain; selected anyway
+    (m_eff too large, or a NaN in a masked-out entry), its value propagates.  The float64 distance sums depend on the
+    reduction order, so a GPU distance can differ from this one in its last bits; when no two compared scores are that
+    close the selection is the same, and then the result is bit-identical (the average has a fixed order).  Slots with
+    n = 0 keep θ_m.  Returns the per-slot participant counts ``[M]`` (float32)."""
+    f, m_keep = krum_params(f, m)
+    C, M, P = uploads.shape
+    dev = uploads.device
+    part = n.detach().reshape(C, M).to(dev) > 0
+    counts = part.sum(0).to(torch.float32)
+    keep = None if mask is None else mask.reshape(-1)[:P].to(dev, torch.bool)
+    chunk = 1 << 20
+    for s in range(M):
+        idx = part[:, s].nonzero().flatten().tolist()
+        k = len(idx)
+        if k == 0:
+            continue
+        if k == 1:
+            sel = [0]
+        else:
+            D = torch.zeros(k, k, dtype=torch.float64, device=dev)
+            for i in range(k - 1):
+                xi = uploads[idx[i], s].to(torch.float32)
+                for e0 in range(0, P, chunk):
+                    diff = (uploads[idx[i + 1:], s, e0:e0 + chunk].to(torch.float32) - xi[e0:e0 + chunk]).double()
+                    sq = diff * diff
+                    if keep is not None:
+                        sq = torch.where(keep[e0:e0 + chunk], sq, torch.zeros((), dtype=torch.float64, device=dev))
+                    D[i, i + 1:] += sq.sum(1)
+            D = D + D.T
+            D[torch.isnan(D)] = math.inf
+            _, sel = krum_select(D.cpu().tolist(), f, m_keep)
+        v = uploads[idx[sel[0]], s].to(torch.float32).clone()
+        for i in sel[1:]:
+            v = v + uploads[idx[i], s].to(torch.float32)
+        if len(sel) > 1:
+            v = v / torch.tensor(float(len(sel)), dtype=torch.float32, device=dev)
+        theta[s, :P] = v.to(theta.device)
+    return counts.to(theta.device)
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

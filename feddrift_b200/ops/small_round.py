@@ -11,7 +11,7 @@ from . import _ext
 
 KIND_ID = {"lr": 0, "fnn": 1}
 MODE_ID = {"pool": 0, "time": 1, "index": 2}
-AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2, "geometric_median": 3}
+AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2, "geometric_median": 3, "multi_krum": 4}
 LAUNCH_COUNT = {"fed_round_small": 0}
 
 
@@ -25,7 +25,8 @@ def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, s
     """True when the fused kernel can run this federation at time step ``t_cur`` (instantiated MLP shape, ``t_cur`` below
     the kernel's plan-table limit, shared-memory layout — plus the ``[2, M, P]`` server optimizer state when
     ``server_opt`` — within 227 KB, and with a ``robust`` aggregation rule 2·C ≤ 33·P for the ranking scratch; ``rule``
-    'geometric_median' (implies ``robust``) also needs a slot's C uploads and weights in the CTA's gradient buffers);
+    'geometric_median' (implies ``robust``) also needs a slot's C uploads and weights in the CTA's gradient buffers, and
+    'multi_krum' a slot's C uploads with per-warp distance rows in them);
     otherwise route to the generic executor."""
     ext = _ext.load()
     if ext is None:
@@ -163,9 +164,10 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
     elif compression != "none":
         from .reference import compression_params
         compression_params(compression, 16, 512)   # raises for an unknown compression
-    from .reference import aggregation_params, geomed_params
+    from .reference import aggregation_params, geomed_params, krum_params
     rule, beta = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
     gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
+    krum_f, krum_m = krum_params(st.get("krum_f", 1), st.get("krum_m", 1))
     if rule != "mean":   # robust aggregation rule (reference.fed_round_small documents the keys)
         if mg:
             raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only")
@@ -173,6 +175,8 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         fcfg += [float(AGG_RULE_ID[rule]), beta]
         if rule == "geometric_median":
             fcfg += [float(gm_iters), gm_nu]
+        elif rule == "multi_krum":   # the geometric-median slots 16..17 are unread
+            fcfg += [4.0, 1e-6, float(krum_f), float(krum_m)]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out

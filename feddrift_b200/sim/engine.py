@@ -36,8 +36,8 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, compression_params, geomed_params, prox_mu_param, qsgd_upload_bits,
-                             topk_k, topk_ratio_param, topk_upload_bits)
+from ..ops.reference import (aggregation_params, compression_params, geomed_params, krum_params, prox_mu_param,
+                             qsgd_upload_bits, topk_k, topk_ratio_param, topk_upload_bits)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -54,7 +54,7 @@ DEFAULTS = dict(
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
     compression="none", quantize_level=16, quantize_bucket=512, topk_ratio=0.01,
-    aggregation_rule="mean", trim_ratio=0.1, geomed_iters=4, geomed_nu=1e-6,
+    aggregation_rule="mean", trim_ratio=0.1, geomed_iters=4, geomed_nu=1e-6, krum_f=1, krum_m=1,
 )
 
 
@@ -118,7 +118,16 @@ class DriftSim:
         rule, beta = aggregation_params(getattr(args, "aggregation_rule", "mean") or "mean", getattr(args, "trim_ratio", 0.1))
         # the geometric median (--geomed_iters R / --geomed_nu ν, validated whatever the rule) carries (rule, β, R, ν)
         gm_iters, gm_nu = geomed_params(getattr(args, "geomed_iters", 4), getattr(args, "geomed_nu", 1e-6))
-        self.agg_rule = None if rule == "mean" else ((rule, beta, gm_iters, gm_nu) if rule == "geometric_median" else (rule, beta))
+        # Multi-Krum (--krum_f f / --krum_m m, validated whatever the rule) carries (rule, β, f, m)
+        krum_f, krum_m = krum_params(getattr(args, "krum_f", 1), getattr(args, "krum_m", 1))
+        if rule == "mean":
+            self.agg_rule = None
+        elif rule == "geometric_median":
+            self.agg_rule = (rule, beta, gm_iters, gm_nu)
+        elif rule == "multi_krum":
+            self.agg_rule = (rule, beta, krum_f, krum_m)
+        else:
+            self.agg_rule = (rule, beta)
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -249,6 +258,8 @@ class DriftSim:
                 self._small.update(aggregation_rule=self.agg_rule[0], trim_ratio=self.agg_rule[1])
                 if self.agg_rule[0] == "geometric_median":
                     self._small.update(geomed_iters=self.agg_rule[2], geomed_nu=self.agg_rule[3])
+                elif self.agg_rule[0] == "multi_krum":
+                    self._small.update(krum_f=self.agg_rule[2], krum_m=self.agg_rule[3])
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)

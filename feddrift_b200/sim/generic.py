@@ -15,7 +15,7 @@ architecture and for algorithms that must look at raw client updates before aggr
   trained rows in place (``ops.qsgd_slots_``, K17) right after local training, so the hooks see the quantized uploads;
   top-k with error feedback sparsifies them there instead (``ops.eftopk_slots_``, K18, residual ``ClientArena.ef_res``);
   a robust aggregation rule (``sim.agg_rule``) makes the same call take the coordinate-wise median / trimmed mean (K19)
-  or the geometric median (K20, distances over the trainable entries ``sim.defense_mask``);
+  or the geometric median (K20) or Multi-Krum (K21), both with distances over the trainable entries ``sim.defense_mask``;
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -145,7 +145,7 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
                 _peer_aggregate(sim, world, rank)
             else:
                 rule = getattr(sim, "agg_rule", None)
-                if rule is not None and rule[0] == "geometric_median":
+                if rule is not None and rule[0] in ("geometric_median", "multi_krum"):
                     ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule, mask=sim.defense_mask)
                 else:
                     ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule)
