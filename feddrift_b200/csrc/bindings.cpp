@@ -29,7 +29,7 @@ std::vector<int64_t> fed_round_small(
     std::vector<double> fcfg, std::vector<int64_t> icfg, std::vector<int64_t> peer_inbox,
     c10::optional<Tensor> error_flag, c10::optional<Tensor> counters, std::vector<int64_t> peer_metrics, std::vector<int64_t> host_io,
     c10::optional<Tensor> participation, c10::optional<Tensor> server_s0, c10::optional<Tensor> server_s1,
-    c10::optional<Tensor> server_step, c10::optional<Tensor> ef_res) {
+    c10::optional<Tensor> server_step, c10::optional<Tensor> ef_res, c10::optional<Tensor> attack_mask) {
     CHECK_CUDA_F32(X); CHECK_CUDA_I32(Y); CHECK_CUDA_I32(nsamp); CHECK_CUDA_F32(W); CHECK_CUDA_F32(theta); CHECK_CUDA_I32(opt_step);
     CHECK_CUDA_F32(metrics);
     TORCH_CHECK(X.is_contiguous() && Y.is_contiguous() && nsamp.is_contiguous() && W.is_contiguous() && metrics.is_contiguous(),
@@ -179,10 +179,30 @@ std::vector<int64_t> fed_round_small(
             TORCH_CHECK(p.world == 1, "fed_round_small: a robust aggregation rule is single-GPU only");
             TORCH_CHECK(2 * (int64_t)p.C <= 33 * theta.size(1),
                         "fed_round_small: too many clients for the robust aggregation scratch (use fed_round_small_fits to route)");
-            TORCH_CHECK(p.agg_rule != 3 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 3),
+            TORCH_CHECK(p.agg_rule != 3 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 3, 0),
                         "fed_round_small: too many clients for the geometric-median scratch (use fed_round_small_fits to route)");
-            TORCH_CHECK(p.agg_rule != 4 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 4),
+            TORCH_CHECK(p.agg_rule != 4 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 4, 0),
                         "fed_round_small: too many clients for the Multi-Krum scratch (use fed_round_small_fits to route)");
+        }
+    }
+    if (fcfg.size() >= 22) {   // simulated Byzantine clients: fcfg[20] = attack kind (0 none, 1 sign_flip, 2 gaussian),
+                               // fcfg[21] = scale, attack_mask [C] uint8 the attackers
+        const double kd = fcfg[20], s = fcfg[21];
+        TORCH_CHECK(kd == 0.0 || kd == 1.0 || kd == 2.0,
+                    "fed_round_small: attack kind must be 0 (none), 1 (sign_flip) or 2 (gaussian); alie and ipm run on the generic "
+                    "executor (use fed_round_small_fits to route)");
+        p.attack_kind = (int)kd;
+        if (p.attack_kind != 0) {
+            TORCH_CHECK(std::isfinite(s) && s > 0.0 && std::isfinite((float)s) && (float)s > 0.f,
+                        "fed_round_small: attack_scale must be finite and > 0 in float32");
+            TORCH_CHECK(p.world == 1, "fed_round_small: a simulated attack is single-GPU only");
+            TORCH_CHECK(attack_mask.has_value() && attack_mask->defined(), "fed_round_small: an attack needs attack_mask");
+            const Tensor& am = *attack_mask;
+            TORCH_CHECK(am.is_cuda() && am.device() == X.device() && am.scalar_type() == torch::kUInt8 && am.is_contiguous() &&
+                            am.numel() == p.C,
+                        "fed_round_small: attack_mask must be a contiguous uint8 [C] tensor on the device of X");
+            p.attack_scale = (float)s;
+            p.attack_mask = am.data_ptr<uint8_t>();
         }
     }
     fdb::SmallLaunchInfo info{};
@@ -193,10 +213,12 @@ std::vector<int64_t> fed_round_small(
     return {info.cluster, info.threads, info.smem_bytes};
 }
 
-// agg_rule: 0 mean, 1 median, 2 trimmed mean, 3 geometric median, 4 Multi-Krum (the scratch each rule needs)
+// agg_rule: 0 mean, 1 median, 2 trimmed mean, 3 geometric median, 4 Multi-Krum (the scratch each rule needs); attack_kind:
+// 0 none, 1 sign_flip, 2 gaussian (in the kernel), 3 alie, 4 ipm (never: the generic executor runs them)
 bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur, bool server_opt,
-                          int64_t agg_rule) {
-    return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt, (int)agg_rule) != 0;
+                          int64_t agg_rule, int64_t attack_kind) {
+    return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt, (int)agg_rule,
+                                     (int)attack_kind) != 0;
 }
 
 bool fed_round_small_supported(int64_t kind, int64_t din, int64_t hid, int64_t dout) {
@@ -427,6 +449,41 @@ void eftopk_slots(Tensor rows, Tensor theta, Tensor residual, c10::optional<Tens
     CHECK_OK(fdb::eftopk_slots_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)M, residual.data_ptr<float>(),
                                       np_, mp, (int)R, P, k, reinterpret_cast<unsigned*>(scratch.data_ptr<int>()), cur_stream()),
              "eftopk_slots");
+}
+
+// K22 over an upload arena rows [C, M, P] (contiguous), in place: every attacker pair (attackers[c] != 0, n[c, m] > 0)
+// uploads the poisoned value of kind 1 sign_flip, 2 gaussian, 3 alie or 4 ipm with scale > 0 against its slot's model
+// theta[m, :P] (theta [M, stride >= P], unit column stride) on the entries whose mask byte is nonzero (ops/reference.py
+// attack_slots_).  The gaussian noise is gauss_hash(seed, c·M + m, e).
+void attack_slots(Tensor rows, Tensor theta, Tensor n, Tensor attackers, int64_t kind, double scale, c10::optional<Tensor> mask,
+                  int64_t seed) {
+    CHECK_CUDA_F32(rows); CHECK_CUDA_F32(theta); CHECK_CUDA_F32(n);
+    TORCH_CHECK(rows.is_contiguous() && rows.dim() == 3, "attack_slots: rows must be a contiguous [C, M, P] tensor");
+    const int64_t C = rows.size(0), M = rows.size(1), P = rows.size(2);
+    TORCH_CHECK(kind >= 1 && kind <= 4, "attack_slots: kind must be 1 (sign_flip), 2 (gaussian), 3 (alie) or 4 (ipm)");
+    TORCH_CHECK(std::isfinite(scale) && scale > 0.0 && std::isfinite((float)scale) && (float)scale > 0.f,
+                "attack_slots: scale must be finite and > 0 in float32");
+    TORCH_CHECK(seed >= 0 && seed <= 0xFFFFFFFFLL, "attack_slots: seed must be a 32-bit unsigned value");
+    TORCH_CHECK(C * M <= 65535 && M <= 65535, "attack_slots: at most 65535 (client, slot) rows are supported");
+    TORCH_CHECK(theta.device() == rows.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "attack_slots: theta must be [M, >= P] with unit column stride on the device of rows");
+    TORCH_CHECK(n.device() == rows.device() && n.is_contiguous() && n.numel() == C * M,
+                "attack_slots: n must be a contiguous float32 [C, M] tensor on the device of rows");
+    TORCH_CHECK(attackers.is_cuda() && attackers.device() == rows.device() && attackers.scalar_type() == torch::kUInt8 &&
+                    attackers.is_contiguous() && attackers.numel() == C,
+                "attack_slots: attackers must be a contiguous uint8 [C] tensor on the device of rows");
+    const unsigned char* mp = nullptr;
+    if (mask.has_value() && mask->defined()) {
+        TORCH_CHECK(mask->is_cuda() && mask->device() == rows.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                    mask->numel() >= P, "attack_slots: mask must be a contiguous uint8 [>= P] tensor on the device of rows");
+        mp = mask->data_ptr<unsigned char>();
+    }
+    if (C * M == 0 || P == 0) return;
+    c10::cuda::CUDAGuard guard(rows.device());
+    CHECK_OK(fdb::attack_slots_launch(rows.data_ptr<float>(), theta.data_ptr<float>(), theta.stride(0), (int)C, (int)M, P,
+                                      n.data_ptr<float>(), attackers.data_ptr<uint8_t>(), (int)kind, (float)scale, mp,
+                                      (unsigned)seed, cur_stream()),
+             "attack_slots");
 }
 
 // K19: coordinate-wise median (rule 1) or trimmed mean (rule 2, trim ratio beta) of the participants (n[c, m] > 0) of every
@@ -1258,6 +1315,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("robust_clip_slots", &robust_clip_slots);
     m.def("qsgd_slots", &qsgd_slots);
     m.def("eftopk_slots", &eftopk_slots);
+    m.def("attack_slots", &attack_slots);
     m.def("robust_aggregate_slots", &robust_aggregate_slots);
     m.def("geomed_aggregate_slots", &geomed_aggregate_slots);
     m.def("krum_aggregate_slots", &krum_aggregate_slots);

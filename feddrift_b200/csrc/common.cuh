@@ -42,6 +42,16 @@ FDB_HOST_DEVICE float uniform_hash(uint32_t seed, uint32_t r, unsigned long long
 // uniform_hash seed of the QSGD draws of round `rnd` of a time step whose engine seed is `seed` (ops/reference.py
 // compress_seed); its constants differ from defense_seed's so that quantization draws and weak-DP noise are independent
 FDB_HOST_DEVICE uint32_t compress_seed(uint32_t seed, uint32_t rnd) { return mix32(seed ^ mix32(rnd * 0x27D4EB2Fu + 0x165667B1u)); }
+// gauss_hash seed of the gaussian model-poisoning attack of round `rnd` (ops/reference.py attack_seed); constants distinct
+// from defense_seed's and compress_seed's
+FDB_HOST_DEVICE uint32_t attack_seed(uint32_t seed, uint32_t rnd) { return mix32(seed ^ mix32(rnd * 0x85EBCA77u + 0x3C6EF372u)); }
+// attack kinds (ops/reference.py ATTACK_ID) and the upload an elementwise attacker sends for one trainable entry x with
+// round-start model th (sign_flip: th − s·(x − th); gaussian: th + s·xi), every operation rounded on its own
+constexpr int kAttackNone = 0, kAttackSignFlip = 1, kAttackGaussian = 2, kAttackAlie = 3, kAttackIpm = 4;
+FDB_DEVICE float attack_entry(int kind, float x, float th, float s, uint32_t seed, uint32_t r, unsigned long long e) {
+    return kind == kAttackSignFlip ? __fsub_rn(th, __fmul_rn(s, __fsub_rn(x, th)))
+                                   : __fadd_rn(th, __fmul_rn(s, gauss_hash(seed, r, e)));
+}
 // QSGD of one trainable entry x with anchor th, bucket scale sigma > 0, level s and uniform draw u (ops/reference.py
 // qsgd_slots_): a = (|d| / σ)·s, q = floor(a) + (u < frac(a)), x' = th + copysign(σ·(q / s), d) with d = x − th.  Every
 // operation is rounded on its own (no FMA contraction), so the result matches the CPU oracle bit for bit.

@@ -329,11 +329,23 @@ struct BatchSel {
 // upload compression of the publish step (template argument kComp)
 constexpr int kCompNone = 0, kCompQsgd = 1, kCompEfTopk = 2;
 
+// a Byzantine client's upload (sign_flip / gaussian) in the publish step: the leader warp rewrites the group's local model
+// thl against the round-start model th0, lane l owning entries l, l + 32, … as in the rest of the publish step.  Not
+// inlined, so the training loop of the kAttack kernels keeps its register allocation
+template <int P>
+__device__ __noinline__ void attack_upload(float* thl, const float* th0, int kind, float s, unsigned seed, unsigned rnd, uint32_t row,
+                                           int lane) {
+    const uint32_t aseed = attack_seed(seed, rnd);
+    for (int pp = lane; pp < P; pp += 32) thl[pp] = attack_entry(kind, thl[pp], th0[pp], s, aseed, row, (unsigned long long)pp);
+    __syncwarp();
+}
+
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
 // its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kComp: the upload compression
 // (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0) and kRobust: a median / trimmed-mean aggregation rule
-// or geometric median or Multi-Krum (p.agg_rule != 0), separate for the same reason
-template <class Net, bool kDefend, bool kProx, int kComp, bool kRobust>
+// or geometric median or Multi-Krum (p.agg_rule != 0), and kAttack: simulated Byzantine clients (p.attack_kind != 0),
+// separate for the same reason
+template <class Net, bool kDefend, bool kProx, int kComp, bool kRobust, bool kAttack>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
     using Cfg = SmallCfg<Net>;
     constexpr int P = Net::P, IN = Net::kIn, OUT = Net::kOut, HID = Net::kHid;
@@ -738,6 +750,11 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                         }
                     }
                 }
+                // simulated Byzantine client: its upload replaces the compressed local model (θ_s still holds the
+                // round-start models), so client_out, the defense and the aggregation all see the poisoned one
+                if constexpr (kAttack)
+                    if (p.attack_mask[c])
+                        attack_upload<P>(thl, theta_s + m * P, p.attack_kind, p.attack_scale, p.seed, rnd, (uint32_t)k, lane);
                 // a robust rule ranks the uploads themselves: slot_s holds them unweighted (x · 1 == x)
                 const float wgt = kRobust ? 1.f : ncm_s[k] / tot_s[m];
                 float dscale = 1.f;
@@ -1069,16 +1086,18 @@ __global__ void mlp_eval_matrix_kernel(const float* __restrict__ theta, int thet
 }
 
 // ================================================================================ host launchers
-template <class Net, bool kDefend, bool kProx, bool kRobust>
+template <class Net, bool kDefend, bool kProx, bool kRobust, bool kAttack>
 static auto round_kernel_c(int comp) {
-    return comp == kCompEfTopk ? fed_round_small_kernel<Net, kDefend, kProx, kCompEfTopk, kRobust>
-         : comp == kCompQsgd   ? fed_round_small_kernel<Net, kDefend, kProx, kCompQsgd, kRobust>
-                               : fed_round_small_kernel<Net, kDefend, kProx, kCompNone, kRobust>;
+    return comp == kCompEfTopk ? fed_round_small_kernel<Net, kDefend, kProx, kCompEfTopk, kRobust, kAttack>
+         : comp == kCompQsgd   ? fed_round_small_kernel<Net, kDefend, kProx, kCompQsgd, kRobust, kAttack>
+                               : fed_round_small_kernel<Net, kDefend, kProx, kCompNone, kRobust, kAttack>;
 }
 
 template <class Net, bool kDefend, bool kProx>
-static auto round_kernel(int comp, bool robust) {
-    return robust ? round_kernel_c<Net, kDefend, kProx, true>(comp) : round_kernel_c<Net, kDefend, kProx, false>(comp);
+static auto round_kernel(int comp, bool robust, bool attack) {
+    return attack ? (robust ? round_kernel_c<Net, kDefend, kProx, true, true>(comp) : round_kernel_c<Net, kDefend, kProx, false, true>(comp))
+                  : (robust ? round_kernel_c<Net, kDefend, kProx, true, false>(comp)
+                            : round_kernel_c<Net, kDefend, kProx, false, false>(comp));
 }
 
 template <class Net>
@@ -1099,9 +1118,10 @@ static int launch_round(const RoundParams& p, int cluster, cudaStream_t stream, 
     if (smem > 227 * 1024) return -2;
     const bool defend = p.def_bound > 0.f, prox = p.prox_mu > 0.f;
     const int comp = p.topk_k > 0 ? kCompEfTopk : (p.q_level > 0 ? kCompQsgd : kCompNone);
-    const bool robust = p.agg_rule != 0;
-    auto kern = prox ? (defend ? round_kernel<Net, true, true>(comp, robust) : round_kernel<Net, false, true>(comp, robust))
-                     : (defend ? round_kernel<Net, true, false>(comp, robust) : round_kernel<Net, false, false>(comp, robust));
+    const bool robust = p.agg_rule != 0, attack = p.attack_kind != 0;
+    auto kern = prox ? (defend ? round_kernel<Net, true, true>(comp, robust, attack) : round_kernel<Net, false, true>(comp, robust, attack))
+                     : (defend ? round_kernel<Net, true, false>(comp, robust, attack)
+                               : round_kernel<Net, false, false>(comp, robust, attack));
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return -3;
     cudaLaunchConfig_t cfg{};
@@ -1141,9 +1161,10 @@ static int fits_round(int C, int M, bool server_opt) {
 // optimizer state when server_opt) within 227 KB, and under a robust aggregation rule (agg_rule 1..4) 2·C ≤ 33·P (a slot's
 // uploads and their ranked copy fit the ranking warp's gbuf); the geometric median (3) also needs C·(P + 2) + 4 ≤ the
 // CTA's gbuf (a slot's uploads, weights and pair list), Multi-Krum (4) C·(P + 4·warps + 4) + 4 ≤ it (a slot's uploads,
-// per-warp fp64 distance and sorted rows, fp64 scores, pair list and selection flags)
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule) {
-    if (t_cur >= kTmax) return 0;
+// per-warp fp64 distance and sorted rows, fp64 scores, pair list and selection flags).  attack_kind 3 (alie) and 4 (ipm)
+// need statistics over other CTAs' pairs before the defense runs, so they go to the generic executor (K22)
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule, int attack_kind) {
+    if (t_cur >= kTmax || attack_kind == kAttackAlie || attack_kind == kAttackIpm) return 0;
 #define FDB_CASE(K, I, H, O)                                                                                            \
     if (kind == K && din == I && (K == 0 || hid == H) && dout == O)                                                     \
         return fits_round<Mlp<K, I, H, O>>(C, M, server_opt) && (agg_rule == 0 || 2 * C <= 33 * Mlp<K, I, H, O>::P) && \

@@ -60,6 +60,12 @@ struct RoundParams {
     // agg_rule 4: Multi-Krum (ops/reference.py krum_aggregate_slots_): the average of the min(krum_m, n) uploads whose
     // summed squared distances to their clamp(n − krum_f − 2, 1, n − 1) nearest neighbours are smallest
     int krum_f, krum_m;
+    // simulated Byzantine clients (attack_kind 0 = off, 1 sign_flip, 2 gaussian; ops/reference.py attack_slots_): after
+    // compression, every pair of a client with attack_mask[c] != 0 uploads θ_m − s·(x − θ_m) or θ_m + s·gauss_hash(
+    // attack_seed(seed, round), c·M + m, e) instead of x, s = attack_scale, before client_out, the defense and the rule
+    int attack_kind;
+    float attack_scale;
+    const unsigned char* attack_mask;   // [C]
     float* client_out; // optional [C, M, P] export of the local models of the LAST round (nullptr = off)
     const float* lr_ptr; // optional device scalar overriding lr
     // outputs
@@ -102,7 +108,8 @@ struct SmallLaunchInfo {
 int fed_round_small_launch(int kind, int din, int hid, int dout, const RoundParams& p, int cluster, cudaStream_t stream,
                            SmallLaunchInfo* info);
 int fed_round_small_supported(int kind, int din, int hid, int dout);
-int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule);
+int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule,
+                         int attack_kind);
 int mlp_eval_matrix_launch(int kind, int din, int hid, int dout, const float* theta, int theta_stride, int M, const float* X,
                            const int* Y, const int* nsamp, int C, int S, float* correct, float* loss, float* sqerr,
                            cudaStream_t stream);

@@ -51,6 +51,12 @@ int krum_aggregate_launch(float* theta, long long t_stride, const float* cp, con
                           int mkeep, const unsigned char* dmask, int opt_kind, float lr, float momentum, float b1, float b2,
                           float eps, float* s0, float* s1, const int* steps, const unsigned char* mask, void* scratch,
                           cudaStream_t stream);
+// attack.cu (K22): simulated Byzantine clients of rows [C, M, P] against theta + m·t_stride: every attacker pair
+// (attackers[c] != 0, n[c·M + m] > 0) uploads the kind's poisoned value (1 sign_flip, 2 gaussian with gauss_hash(seed,
+// c·M + m, e), 3 alie, 4 ipm; scale s > 0) on the entries with mask != 0 (mask may be nullptr).  -5: bad kind or scale
+int attack_slots_launch(float* rows, const float* theta, long long t_stride, int C, int M, long long P, const float* n,
+                        const unsigned char* attackers, int kind, float scale, const unsigned char* mask, unsigned seed,
+                        cudaStream_t stream);
 // aggregate_peer.cu : multi-GPU reduce-scatter + apply + all-gather over NVLink peer memory (cooperative launch)
 int fedavg_reduce_apply_peer_launch(const float* cp, const int* cidx, const float* n, int C, int M, int P, int theta_stride, int world, int rank,
                                     const long long* part_ptrs, const long long* theta_ptrs, const long long* tot_ptrs,

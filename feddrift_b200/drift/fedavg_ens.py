@@ -34,8 +34,8 @@ from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, compress_seed, compression_params, geomed_params, krum_params,
-                             prox_mu_param, topk_k, topk_ratio_param)
+from ..ops.reference import (aggregation_params, attack_params, attack_seed, attacker_clients, compress_seed,
+                             compression_params, geomed_params, krum_params, prox_mu_param, topk_k, topk_ratio_param)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
 from ..utils.metrics import get_sink
@@ -453,6 +453,13 @@ class _BaseAggregator:
             if self.topk_k else None
         self.bank.ef_res = self.ef_res
         self._round_clients = None
+        # simulated Byzantine clients (--attack_type / --attack_clients / --attack_scale, validated whatever the type): the
+        # run's attacker set over CLIENTS; a round's uploads are poisoned once all of them have arrived (the attacker model
+        # sits at the aggregator, as in later FedML releases), rows mapped to clients through client_sampling's list
+        atk, atk_a, atk_s = attack_params(getattr(args, "attack_type", "none") or "none", getattr(args, "attack_clients", 0),
+                                          getattr(args, "attack_scale", 1.0), n_clients)
+        self.attackers = attacker_clients(n_clients, atk_a, int(getattr(args, "dummy_arg", 0)))
+        self.attack = (atk, atk_s) if atk != "none" and atk_a > 0 else None
         self.upload = torch.zeros(worker_num, M, P, dtype=torch.float32, device=self.device)
         self.upload_n = torch.zeros(worker_num, M, dtype=torch.float32, device=self.device)
         self.flag_client_model_uploaded_dict = {i: False for i in range(worker_num)}
@@ -500,8 +507,21 @@ class _BaseAggregator:
             return False
         for i in range(self.worker_num):
             self.flag_client_model_uploaded_dict[i] = False
+        if self.attack is not None:
+            self._attack_uploads()
         self._compress_round += 1
         return True
+
+    def _attack_uploads(self):
+        """Poison the complete round's upload arena in place (``ops.attack_slots_``) before any consumer reads it: row w is
+        worker w, which trained client ``_round_clients[w]`` this round; the noise follows the round counter."""
+        W = self.worker_num
+        clients = self._round_clients if self._round_clients is not None else range(W)
+        rows = torch.tensor([bool(self.attackers[int(c)]) for c in list(clients)[:W]], dtype=torch.bool)
+        a = self.args
+        seed = int(getattr(a, "dummy_arg", 0)) * 7919 + 13 + 1000003 * int(getattr(a, "curr_train_iteration", 0) or 0)
+        ops.attack_slots_(self.upload, self.bank.theta, self.upload_n, rows, self.attack[0], self.attack[1], self.defense_mask,
+                          attack_seed(seed, self._compress_round))
 
     def _aggregate_models(self, model_mask: Optional[np.ndarray] = None):
         n = self.upload_n.clone()

@@ -57,6 +57,13 @@ CONFIGS = {
                                                         concept_drift_algo_arg="H_A_C_1_10_0", concept_num=4, change_points="A",
                                                         sample_num=100, batch_size=500, comm_round=40,
                                                         aggregation_rule="multi_krum", krum_f=1, krum_m=1),
+    # config 2 with 20 colluding ALIE clients ("A Little Is Enough", z = 1) against the coordinate-wise median
+    "cfg2a_sea_fnn_100clients_alie_median_feddrift": dict(model="fnn", dataset="sea", client_num_in_total=100,
+                                                          client_num_per_round=100, concept_drift_algo="softcluster",
+                                                          concept_drift_algo_arg="H_A_C_1_10_0", concept_num=4,
+                                                          change_points="A", sample_num=100, batch_size=500, comm_round=40,
+                                                          aggregation_rule="median", attack_type="alie", attack_clients=20,
+                                                          attack_scale=1.0),
     # config 3: MNIST 2-conv CNN, 4 concepts, 64 clients, IFCA hard-r
     "cfg3_mnist_cnn_64clients_ifca": dict(model="cnn", dataset="MNIST", client_num_in_total=64, client_num_per_round=64,
                                           concept_drift_algo="softclusterwin-1", concept_drift_algo_arg="hard-r", concept_num=4,

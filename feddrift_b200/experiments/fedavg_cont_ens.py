@@ -77,6 +77,11 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     # rule with one name, --krum_m 1 is plain Krum
     a("--krum_f", type=int, default=1, help="multi_krum: Byzantine uploads f assumed per slot, 0..65535")
     a("--krum_m", type=int, default=1, help="multi_krum: uploads m averaged, 1..65535 (1: Krum)")
+    # simulated Byzantine clients: a fixed set of --attack_clients clients poisons its uploads after compression (sign_flip:
+    # the reversed update, gaussian: noise around the model, alie: "A Little Is Enough", ipm: inner-product manipulation)
+    a("--attack_type", type=str, default="none", choices=["none", "sign_flip", "gaussian", "alie", "ipm"])
+    a("--attack_clients", type=int, default=0, help="attack: number a of Byzantine clients, 0..client_num_in_total")
+    a("--attack_scale", type=float, default=1.0, help="attack: strength s > 0 (sign_flip / gaussian scale, ALIE z, IPM ε)")
     # FedProx local training: every client step minimises CE + mu/2‖w − w_m‖², w_m the cluster model it received (0 = off)
     a("--fedprox_mu", type=float, default=0.0)
     # façade extras: worker packing, zero-copy device payloads, straggler tolerance (core.managers.RoundWatchdog)

@@ -22,6 +22,7 @@ Kernel map (SURVEY §2.9 numbering):
   K19 robust_aggregate_slots_ (median / trimmed mean)   csrc/robust_agg.cu
   K20 geomed_aggregate_slots_ (geometric median)        csrc/robust_agg.cu
   K21 krum_aggregate_slots_ (Multi-Krum)                csrc/robust_agg.cu
+  K22 attack_slots_ (simulated Byzantine clients)       csrc/attack.cu
 """
 from __future__ import annotations
 
@@ -207,6 +208,25 @@ def eftopk_slots_(rows, theta, residual, n=None, k: int = 1, weight_mask=None):
         _ext.load().eftopk_slots(rows, theta, residual, nn, int(k), mask)
         return rows
     return ref.eftopk_slots_(rows, theta, residual, n, k, weight_mask)
+
+
+def attack_slots_(rows, theta, n, attackers, kind: str, scale: float = 1.0, mask=None, seed: int = 0):
+    """K22: simulated Byzantine clients of an upload arena ``rows [C, M, P]`` in place: every pair of a client with
+    ``attackers[c]`` (bool [C]) and ``n[c, m] > 0`` uploads the poisoned value of ``kind`` ('sign_flip', 'gaussian' with
+    noise ``gauss_hash(seed, c·M + m, ·)``, 'alie' or 'ipm') with strength ``scale`` against its slot's model
+    ``theta[m, :P]`` (``theta`` may be a padded bank) on the entries of ``mask`` (bool [P], None = all).  'none' is a
+    no-op.  See ``reference.attack_slots_``; returns ``rows``."""
+    kind, _, scale = ref.attack_params(kind, 0, scale, rows.shape[0])
+    if kind == "none":
+        return rows
+    if native(rows, theta):
+        dev = rows.device
+        att = torch.as_tensor(attackers).reshape(-1).to(dev, torch.uint8).contiguous()
+        dm = None if mask is None else mask.reshape(-1)[: rows.shape[2]].to(dev, torch.uint8).contiguous()
+        _ext.load().attack_slots(rows, theta, n.float().contiguous(), att, ref.ATTACK_ID[kind], scale, dm,
+                                 int(seed) & 0xFFFFFFFF)
+        return rows
+    return ref.attack_slots_(rows, theta, n, attackers, kind, scale, mask, seed)
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, **kw):

@@ -228,6 +228,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     rule by ``geomed_params``: the same, with ``geomed_aggregate_slots_`` (every entry is trainable in these MLPs).
     ``aggregation_rule`` 'multi_krum' with ``krum_f`` f (1) and ``krum_m`` m (1), validated whatever the rule by
     ``krum_params``: the same, with ``krum_aggregate_slots_``.
+    ``attack_type`` 'sign_flip'|'gaussian'|'alie'|'ipm' (absent or 'none': off) with ``attack_clients`` a (0) and
+    ``attack_scale`` s (1.0), validated whatever the type by ``attack_params``, and ``attackers`` (bool/uint8 [C], absent:
+    ``attacker_clients(C, a, 0)``, which must hold a clients): after compression and before ``client_out``, the defense
+    and the rule, the uploads go through ``attack_slots_`` with seed ``attack_seed(seed, rnd)``.
     ``fedprox_mu`` (absent or 0: off): every local
     step of pair (c, m) feeds ``prox_grad(g, w, (mu, θ_m, None, None))`` to the client optimizer, θ_m the round-start model
     (FedProx: the local objective gains μ/2‖w − θ_m‖²; Adam adds wd·w after it).
@@ -265,6 +269,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     agg_rule, trim_ratio = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
     gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
     krum_f, krum_m = krum_params(st.get("krum_f", 1), st.get("krum_m", 1))
+    atk_type, atk_a, atk_scale = attack_params(st.get("attack_type") or "none", st.get("attack_clients", 0),
+                                               st.get("attack_scale", 1.0), C)
+    attackers = attack_table(st.get("attackers"), C, atk_a)
+    atk_on = atk_type != "none" and atk_a > 0
     client_out = st.get("client_out")
     for r in range(rounds):
         rnd = round0 + r
@@ -319,6 +327,13 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
             for (c, m), (p, _) in locals_.items():
                 up[c, m], trained[c, m] = p, 1.0
             eftopk_slots_(up, theta, st["ef_residual"], trained, ef_k, None)
+            locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
+        if atk_on and locals_:   # the Byzantine clients replace their uploads as they leave (after compression)
+            up = torch.zeros(C, M, P, dtype=torch.float32)
+            trained = torch.zeros(C, M)
+            for (c, m), (p, _) in locals_.items():
+                up[c, m], trained[c, m] = p, 1.0
+            attack_slots_(up, theta, trained, attackers, atk_type, atk_scale, None, attack_seed(seed, rnd))
             locals_ = {(c, m): (up[c, m], n_cm) for (c, m), (_, n_cm) in locals_.items()}
         if client_out is not None and r == rounds - 1:
             for (c, m), (p, _) in locals_.items():
@@ -950,6 +965,126 @@ def krum_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch.T
             v = v / torch.tensor(float(len(sel)), dtype=torch.float32, device=dev)
         theta[s, :P] = v.to(theta.device)
     return counts.to(theta.device)
+
+
+ATTACK_TYPES = ("none", "sign_flip", "gaussian", "alie", "ipm")
+_F32_ZERO_AT, _F32_INF_AT = 2.0 ** -150, 3.4028235677973366e38   # float32 rounds x ≤ the first to 0, x ≥ the second to inf
+ATTACK_ID = {"none": 0, "sign_flip": 1, "gaussian": 2, "alie": 3, "ipm": 4}
+
+
+def attack_params(attack_type, attack_clients, attack_scale, C: int) -> Tuple[str, int, float]:
+    """Validated ``(--attack_type, --attack_clients, --attack_scale)`` of the simulated Byzantine clients, checked whatever
+    the type: the type is one of ``none``, ``sign_flip``, ``gaussian``, ``alie`` or ``ipm``; a is an int with 0 ≤ a ≤ C
+    (a bool is not an int here); s is a finite number > 0 whose float32 rounding is finite and > 0.  Raises
+    ``ValueError``."""
+    attack_type = "none" if attack_type is None else attack_type
+    if attack_type not in ATTACK_TYPES:
+        raise ValueError(f"attack_type must be one of {', '.join(ATTACK_TYPES)} (got {attack_type!r})")
+    a = attack_clients
+    if isinstance(a, bool) or not isinstance(a, (int, np.integer)) or not 0 <= int(a) <= int(C):
+        raise ValueError(f"attack_clients must be an int in [0, {int(C)}] (got {a!r})")
+    try:
+        s = None if isinstance(attack_scale, bool) else float(attack_scale)
+    except (TypeError, ValueError):
+        s = None
+    # float32 rounds s to a finite value > 0 exactly when 2⁻¹⁵⁰ < s < FLT_MAX + ulp/2 (plain comparisons: this runs on
+    # every fused launch)
+    if s is None or not _F32_ZERO_AT < s < _F32_INF_AT:
+        raise ValueError(f"attack_scale must be a finite number > 0 (got {attack_scale!r})")
+    return attack_type, int(a), s
+
+
+def attacker_clients(C: int, a: int, seed: int) -> torch.Tensor:
+    """The Byzantine clients of a run with seed ``seed`` (``--dummy_arg``): bool ``[C]``, True for the ``a`` clients with
+    the smallest key mix32(seed ^ mix32(c·0x9E3779B9 + 0x85EBCA6B)), ties to the lower index.  The set is fixed for the
+    run (it depends on neither the time step, the round nor client sampling) and nested in ``a``."""
+    C, a = int(C), int(a)
+    keys = [(mix32((seed & M32) ^ mix32((c * 0x9E3779B9 + 0x85EBCA6B) & M32)), c) for c in range(C)]
+    out = torch.zeros(C, dtype=torch.bool)
+    for _, c in sorted(keys)[:a]:
+        out[c] = True
+    return out
+
+
+def attack_table(attackers, C: int, a: int) -> torch.Tensor:
+    """The attacker set of ``fed_round_small``: ``attackers`` (bool/uint8 [C]) when given, which must hold exactly ``a``
+    clients, else ``attacker_clients(C, a, 0)``.  Raises ``ValueError``."""
+    if attackers is None:
+        return attacker_clients(C, a, 0)
+    att = torch.as_tensor(attackers).detach().cpu().reshape(-1).bool()
+    if att.numel() != int(C) or int(att.sum()) != int(a):
+        raise ValueError(f"attackers must be a [C = {int(C)}] table of exactly attack_clients = {int(a)} clients")
+    return att
+
+
+def attack_seed(seed: int, rnd: int) -> int:
+    """``gauss_hash`` seed of the ``gaussian`` attack in round ``rnd`` of a time step whose engine seed is ``seed`` (the
+    ``attack_seed`` of csrc/common.cuh): a function of (seed, round) only, with constants that differ from those of
+    ``defense_seed`` and ``compress_seed``."""
+    return mix32((seed & M32) ^ mix32((rnd * 0x85EBCA77 + 0x3C6EF372) & M32))
+
+
+def attack_slots_(rows: torch.Tensor, theta: torch.Tensor, n, attackers, attack_type: str, scale: float,
+                  weight_mask=None, seed: int = 0) -> torch.Tensor:
+    """Model poisoning (K22) of an upload arena ``rows [C, M, P]``, in place.  For every slot m, with θ = ``theta[m, :P]``
+    (``theta`` may be a padded bank) and s = fl32(``scale``), every attacker pair (``attackers[c]``, ``n[c, m] > 0``)
+    uploads, on each entry e with ``weight_mask`` True (None = all; BatchNorm statistics keep the attacker's values):
+
+    * ``sign_flip``: θ − fl32(s·fl32(x − θ)), its own update reversed and scaled by s;
+    * ``gaussian``: θ + fl32(s·ξ), ξ = ``gauss_hash(seed, c·M + m, e)``;
+    * ``alie``: μ − fl32(s·σ) (A Little Is Enough, Baruch et al. 2019; s is their z);
+    * ``ipm``: θ − fl32(s·fl32(μ − θ)) (inner-product manipulation, Xie et al. 2019; s is their ε).
+
+    μ is the fp32 sum, from 0 in client order, of the honest uploads of the slot (c not an attacker, n[c, m] > 0), divided
+    once by their number h; σ = sqrt_rn(fl32(Σ fl32(δ·δ)) / h) with δ = fl32(x − μ), summed from 0 in client order (the
+    population standard deviation).  Every operation is rounded on its own.  The attackers of a slot collude under
+    ``alie`` and ``ipm``: they upload the same vector; with h = 0 their rows are left as trained.  Pairs with n ≤ 0 and
+    honest pairs are untouched.  Returns ``rows``."""
+    C, M, P = rows.shape
+    attack_type, _, scale = attack_params(attack_type, 0, scale, C)
+    if attack_type == "none" or C * M == 0 or P == 0:
+        return rows
+    dev = rows.device
+    th = theta[:, :P].to(dev, torch.float32)
+    sel = torch.ones(C, M, dtype=torch.bool) if n is None else (n.detach().cpu().reshape(C, M) > 0)
+    att = torch.as_tensor(attackers).detach().cpu().reshape(-1).bool()
+    if att.numel() != C:
+        raise ValueError(f"attack_slots_: attackers must have C = {C} entries (got {att.numel()})")
+    wm = None if weight_mask is None else weight_mask.reshape(-1)[:P].to(dev).bool()
+    sf = torch.tensor(scale, dtype=torch.float32, device=dev)
+    for m in range(M):
+        bad = [c for c in range(C) if bool(att[c]) and bool(sel[c, m])]
+        if not bad:
+            continue
+        if attack_type in ("alie", "ipm"):
+            good = [c for c in range(C) if not bool(att[c]) and bool(sel[c, m])]
+            if not good:
+                continue
+            hf = torch.tensor(float(len(good)), dtype=torch.float32, device=dev)
+            acc = torch.zeros(P, dtype=torch.float32, device=dev)
+            for c in good:
+                acc = acc + rows[c, m]
+            mu = acc / hf
+            if attack_type == "alie":
+                ss = torch.zeros(P, dtype=torch.float32, device=dev)
+                for c in good:
+                    d = rows[c, m] - mu
+                    ss = ss + d * d
+                # sqrt_rn: the float64 root of a float32 rounds to the correctly rounded float32 root (torch's float32
+                # CPU sqrt is not always correctly rounded)
+                crafted = mu - sf * torch.sqrt((ss / hf).double()).float()
+            else:
+                crafted = th[m] - sf * (mu - th[m])
+        for c in bad:
+            row = rows[c, m]
+            if attack_type == "sign_flip":
+                new = th[m] - sf * (row - th[m])
+            elif attack_type == "gaussian":
+                new = th[m] + sf * gauss_hash_rows(seed, [c * M + m], P)[0].to(dev)
+            else:
+                new = crafted
+            row.copy_(new if wm is None else torch.where(wm, new, row))
+    return rows
 
 
 def server_opt_step_(theta, avg, state: Dict, opt: str, lr: float, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8):

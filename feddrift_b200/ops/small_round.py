@@ -8,6 +8,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _ext
+from .reference import ATTACK_ID, attack_params, attack_table
 
 KIND_ID = {"lr": 0, "fnn": 1}
 MODE_ID = {"pool": 0, "time": 1, "index": 2}
@@ -21,18 +22,20 @@ def supported(kind: str, din: int, hid: int, dout: int) -> bool:
 
 
 def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, server_opt: bool = False,
-         robust: bool = False, rule: Optional[str] = None) -> bool:
+         robust: bool = False, rule: Optional[str] = None, attack: Optional[str] = None) -> bool:
     """True when the fused kernel can run this federation at time step ``t_cur`` (instantiated MLP shape, ``t_cur`` below
     the kernel's plan-table limit, shared-memory layout — plus the ``[2, M, P]`` server optimizer state when
     ``server_opt`` — within 227 KB, and with a ``robust`` aggregation rule 2·C ≤ 33·P for the ranking scratch; ``rule``
     'geometric_median' (implies ``robust``) also needs a slot's C uploads and weights in the CTA's gradient buffers, and
-    'multi_krum' a slot's C uploads with per-warp distance rows in them);
-    otherwise route to the generic executor."""
+    'multi_krum' a slot's C uploads with per-warp distance rows in them); the ``attack`` types 'alie' and 'ipm' need
+    statistics over every upload of a slot before the defense, so they never fit ('sign_flip' and 'gaussian' run in the
+    publish step); otherwise route to the generic executor."""
     ext = _ext.load()
     if ext is None:
         return True   # CPU reference has no such limits
     rid = AGG_RULE_ID[rule] if rule not in (None, "mean") else (1 if robust else 0)
-    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt), rid))
+    return bool(ext.fed_round_small_fits(KIND_ID[kind], din, hid, dout, int(C), int(M), int(t_cur), bool(server_opt), rid,
+                                         ATTACK_ID[attack or "none"]))
 
 
 def spin_timeout_ms(st: Dict) -> int:
@@ -177,6 +180,18 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
             fcfg += [float(gm_iters), gm_nu]
         elif rule == "multi_krum":   # the geometric-median slots 16..17 are unread
             fcfg += [4.0, 1e-6, float(krum_f), float(krum_m)]
+    atk, atk_a, atk_s = attack_params(st.get("attack_type") or "none", st.get("attack_clients", 0), st.get("attack_scale", 1.0),
+                                      C)
+    attack_mask = None
+    if atk != "none" and atk_a > 0:   # simulated Byzantine clients in the publish step (reference.fed_round_small)
+        if mg:
+            raise ValueError("a simulated attack (--attack_type) is single-GPU only")
+        attack_mask = cache.get("attack_mask")
+        if attack_mask is None:
+            attack_mask = cache["attack_mask"] = attack_table(st.get("attackers"), C, atk_a).to(dev, torch.uint8).contiguous()
+        # server optimizer ... Multi-Krum slots, unread when off (the rule slots hold the mean and valid parameters)
+        fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.1, 4.0, 1e-6, 1.0, 1.0][len(fcfg) - 5:]
+        fcfg += [float(ATTACK_ID[atk]), atk_s]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out
@@ -190,7 +205,7 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         list(mg["inbox_ptrs"]) if mg else [], mg.get("error_flag") if mg else None,
         st.get("counters"), peer_metrics, [int(v) for v in st["host_io"]] if st.get("host_io") else [],
         cache["participation"], st.get("server_s0") if sopt else None, st.get("server_s1") if sopt else None,
-        st.get("server_step") if sopt else None, ef_res)
+        st.get("server_step") if sopt else None, ef_res, attack_mask)
     if mg:
         mg["flag_base"] = int(mg["flag_base"]) + rounds
     if st.get("counters") is not None:

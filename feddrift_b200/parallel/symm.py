@@ -31,6 +31,8 @@ def attach_multi_gpu(sim, world: int, rank: int) -> None:
         raise ValueError("a server optimizer (--server_optimizer) is single-GPU only: attach_multi_gpu refuses it")
     if getattr(sim, "agg_rule", None) is not None:
         raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only: attach_multi_gpu refuses it")
+    if getattr(sim, "attack", None) is not None:
+        raise ValueError("a simulated attack (--attack_type) is single-GPU only: attach_multi_gpu refuses it")
     MP = sim.M * sim.bank.P
     inbox_floats = 2 * (2 * world * MP)                      # 8-byte LL words
     inbox_floats = (inbox_floats + 31) // 32 * 32            # staging area starts on its own 128-byte line

@@ -36,8 +36,8 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, compression_params, geomed_params, krum_params, prox_mu_param,
-                             qsgd_upload_bits, topk_k, topk_ratio_param, topk_upload_bits)
+from ..ops.reference import (aggregation_params, attack_params, attacker_clients, compression_params, geomed_params,
+                             krum_params, prox_mu_param, qsgd_upload_bits, topk_k, topk_ratio_param, topk_upload_bits)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -55,6 +55,7 @@ DEFAULTS = dict(
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
     compression="none", quantize_level=16, quantize_bucket=512, topk_ratio=0.01,
     aggregation_rule="mean", trim_ratio=0.1, geomed_iters=4, geomed_nu=1e-6, krum_f=1, krum_m=1,
+    attack_type="none", attack_clients=0, attack_scale=1.0,
 )
 
 
@@ -128,6 +129,14 @@ class DriftSim:
             self.agg_rule = (rule, beta, krum_f, krum_m)
         else:
             self.agg_rule = (rule, beta)
+        # simulated Byzantine clients (--attack_type / --attack_clients a / --attack_scale s, validated whatever the type):
+        # the a clients of attacker_clients (fixed for the run) poison their uploads after compression; attack = (type, s)
+        # when the type is not 'none' and a > 0, else None
+        atk, atk_a, atk_s = attack_params(getattr(args, "attack_type", "none") or "none", getattr(args, "attack_clients", 0),
+                                          getattr(args, "attack_scale", 1.0), self.C)
+        self.attackers = attacker_clients(self.C, atk_a, seed)
+        self.attack = (atk, atk_s) if atk != "none" and atk_a > 0 else None
+        self._attackers_dev = self.attackers.to(self.device, torch.uint8) if self.attack else None
         self.spec = self.bank.mlp
         self.evaluator = Evaluator(self.bank, self.data, args.batch_size)
         self.t = -1
@@ -260,6 +269,9 @@ class DriftSim:
                     self._small.update(geomed_iters=self.agg_rule[2], geomed_nu=self.agg_rule[3])
                 elif self.agg_rule[0] == "multi_krum":
                     self._small.update(krum_f=self.agg_rule[2], krum_m=self.agg_rule[3])
+            if self.attack is not None:
+                self._small.update(attack_type=self.attack[0], attack_clients=int(self.attackers.sum()),
+                                   attack_scale=self.attack[1], attackers=self._attackers_dev)
             if getattr(self, "multi", None) is not None:
                 self._small["multi_gpu"] = self.multi
             if self.device.type == "cuda":  # device-resident round / epoch counters (CUDA-graph replay friendly)
@@ -279,6 +291,9 @@ class DriftSim:
         if self.agg_rule is not None and (self.multi is not None or getattr(self, "shard_clients", False)):
             raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only: an order statistic needs every "
                              "upload on one device, so it cannot be combined with multi-GPU client sharding")
+        if self.attack is not None and (self.multi is not None or getattr(self, "shard_clients", False)):
+            raise ValueError("a simulated attack (--attack_type) is single-GPU only: ALIE and IPM need every upload of a slot on "
+                             "one device, so it cannot be combined with multi-GPU client sharding")
         done, last = 0, {}
         while done < rounds:
             block = self.algo.block_size(self.round_in_step, rounds - done)
@@ -315,7 +330,8 @@ class DriftSim:
         s = self.spec
         return small_round.fits(s["kind"], s["in"], s["hidden"], s["out"], self.C, self.M, self.t,
                                 server_opt=self.bank.server_opt is not None, robust=self.agg_rule is not None,
-                                rule=None if self.agg_rule is None else self.agg_rule[0])
+                                rule=None if self.agg_rule is None else self.agg_rule[0],
+                                attack=None if self.attack is None else self.attack[0])
 
     def upload_bits(self) -> int:
         """Size in bits of one compressed upload of this federation (``reference.qsgd_upload_bits`` under QSGD,
@@ -509,11 +525,22 @@ class DriftSim:
         tot = m.sum(0).tolist()     # one reduction over the [C, 4] host buffer
         res = {"round": self.round_in_step - 1, "iteration": t, "train_acc": tot[0] / ntr, "train_loss": tot[1] / ntr,
                "test_acc": tot[2] / nte, "test_loss": tot[3] / nte}
+        if self.attack is not None:
+            res["train_acc_honest"], res["test_acc_honest"] = self._honest_acc(m, self._last_counts.cpu().numpy())
         if log:
             for k_, key in (("train_acc", "Train/Acc"), ("train_loss", "Train/Loss"), ("test_acc", "Test/Acc"),
-                            ("test_loss", "Test/Loss")):
-                self.sink.log({key: res[k_], "round": res["round"]})
+                            ("test_loss", "Test/Loss"), ("train_acc_honest", "Train/AccHonest"),
+                            ("test_acc_honest", "Test/AccHonest")):
+                if k_ in res:
+                    self.sink.log({key: res[k_], "round": res["round"]})
         return res
+
+    def _honest_acc(self, m, cnt):
+        """(train, test) accuracy over the clients that are not attackers: their correct predictions over their sample
+        counts, from one round's per-client rows ``m [C, 4]`` and counts ``cnt [C, 2]``."""
+        h = ~self.attackers.numpy()
+        return (float(m[h, 0].sum()) / max(float(cnt[h, 0].sum()), 1.0),
+                float(m[h, 2].sum()) / max(float(cnt[h, 1].sum()), 1.0))
 
     def _flush_metrics(self, out: Dict[str, torch.Tensor], r0: int, n: int) -> Dict:
         """One D2H copy per block; emits the reference's wandb keys for every tested round."""
@@ -539,6 +566,11 @@ class DriftSim:
             self.sink.log({"Test/Loss": te_loss, "round": r})
             last = {"round": r, "train_acc": tr_acc, "train_loss": tr_loss, "test_acc": te_acc,
                     "test_loss": te_loss, "iteration": self.t}
+            if self.attack is not None:   # the honest clients' accuracy, the figure a robust rule is judged by
+                tr_h, te_h = self._honest_acc(met[i], cnt)
+                self.sink.log({"Train/AccHonest": tr_h, "round": r})
+                self.sink.log({"Test/AccHonest": te_h, "round": r})
+                last["test_acc_honest"] = te_h
         if last:
             self.history.append(last)
         return last

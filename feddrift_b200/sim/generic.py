@@ -14,6 +14,8 @@ architecture and for algorithms that must look at raw client updates before aggr
   (``ops.robust_clip_slots_``, K10) after the raw-update hooks have seen them; QSGD upload compression quantizes the
   trained rows in place (``ops.qsgd_slots_``, K17) right after local training, so the hooks see the quantized uploads;
   top-k with error feedback sparsifies them there instead (``ops.eftopk_slots_``, K18, residual ``ClientArena.ef_res``);
+  simulated Byzantine clients (``sim.attack``) then replace their uploads in place (``ops.attack_slots_``, K22, clients
+  ``sim.attackers``, entries ``sim.defense_mask``), so the hooks, the defense and the rule see the poisoned ones;
   a robust aggregation rule (``sim.agg_rule``) makes the same call take the coordinate-wise median / trimmed mean (K19)
   or the geometric median (K20) or Multi-Krum (K21), both with distances over the trainable entries ``sim.defense_mask``;
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
@@ -35,7 +37,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import ops
-from ..ops.reference import batch_hash, compress_seed, mix32
+from ..ops.reference import attack_seed, batch_hash, compress_seed, mix32
 
 
 def _pair_sampler(st: Dict, c: int, m: int, t: int, nb: torch.Tensor, B: int):
@@ -117,6 +119,9 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
             ops.qsgd_slots_(cl.params, bank.theta, cl.n, sim.q_level, sim.q_bucket, sim.defense_mask, compress_seed(seed, rnd))
         if sim.topk_k:   # top-k with error feedback: each client sparsifies its upload and keeps the rest in its residual
             ops.eftopk_slots_(cl.params, bank.theta, cl.ef_res, cl.n, sim.topk_k, sim.defense_mask)
+        if sim.attack is not None:   # the Byzantine clients replace their uploads as they leave, after compression
+            ops.attack_slots_(cl.params, bank.theta, cl.n, sim._attackers_dev, sim.attack[0], sim.attack[1], sim.defense_mask,
+                              attack_seed(seed, rnd))
         # raw-update hooks (CFL family) may veto the aggregation of this round
         skip = False
         wants_raw = (hasattr(sim.algo, "state") and "cfl" in getattr(sim.algo, "arg", "")) or \
