@@ -29,7 +29,8 @@ std::vector<int64_t> fed_round_small(
     std::vector<double> fcfg, std::vector<int64_t> icfg, std::vector<int64_t> peer_inbox,
     c10::optional<Tensor> error_flag, c10::optional<Tensor> counters, std::vector<int64_t> peer_metrics, std::vector<int64_t> host_io,
     c10::optional<Tensor> participation, c10::optional<Tensor> server_s0, c10::optional<Tensor> server_s1,
-    c10::optional<Tensor> server_step, c10::optional<Tensor> ef_res, c10::optional<Tensor> attack_mask) {
+    c10::optional<Tensor> server_step, c10::optional<Tensor> ef_res, c10::optional<Tensor> attack_mask,
+    c10::optional<Tensor> cc_center) {
     CHECK_CUDA_F32(X); CHECK_CUDA_I32(Y); CHECK_CUDA_I32(nsamp); CHECK_CUDA_F32(W); CHECK_CUDA_F32(theta); CHECK_CUDA_I32(opt_step);
     CHECK_CUDA_F32(metrics);
     TORCH_CHECK(X.is_contiguous() && Y.is_contiguous() && nsamp.is_contiguous() && W.is_contiguous() && metrics.is_contiguous(),
@@ -152,12 +153,12 @@ std::vector<int64_t> fed_round_small(
             p.ef_res = er.data_ptr<float>();
         }
     }
-    if (fcfg.size() >= 16) {   // aggregation rule: fcfg[14] = 0 mean / 1 median / 2 trimmed mean / 3 geometric median / 4 Multi-Krum,
-                               // fcfg[15] = trim ratio
+    if (fcfg.size() >= 16) {   // aggregation rule: fcfg[14] = 0 mean / 1 median / 2 trimmed mean / 3 geometric median / 4 Multi-Krum /
+                               // 5 centered clipping, fcfg[15] = trim ratio
         const double rule = fcfg[14], beta = fcfg[15];
-        TORCH_CHECK(rule == 0.0 || rule == 1.0 || rule == 2.0 || rule == 3.0 || rule == 4.0,
-                    "fed_round_small: aggregation rule must be 0 (mean), 1 (median), 2 (trimmed_mean), 3 (geometric_median) or 4 "
-                    "(multi_krum)");
+        TORCH_CHECK(rule == 0.0 || rule == 1.0 || rule == 2.0 || rule == 3.0 || rule == 4.0 || rule == 5.0,
+                    "fed_round_small: aggregation rule must be 0 (mean), 1 (median), 2 (trimmed_mean), 3 (geometric_median), 4 "
+                    "(multi_krum) or 5 (centered_clip)");
         TORCH_CHECK(std::isfinite(beta) && beta >= 0.0 && beta < 0.5, "fed_round_small: trim_ratio must be in [0, 0.5)");
         p.agg_rule = (int)rule; p.trim_ratio = (float)beta;
         if (p.agg_rule == 3) {   // fcfg[16] = Weiszfeld iterations R, fcfg[17] = smoothing nu
@@ -183,6 +184,8 @@ std::vector<int64_t> fed_round_small(
                         "fed_round_small: too many clients for the geometric-median scratch (use fed_round_small_fits to route)");
             TORCH_CHECK(p.agg_rule != 4 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 4, 0),
                         "fed_round_small: too many clients for the Multi-Krum scratch (use fed_round_small_fits to route)");
+            TORCH_CHECK(p.agg_rule != 5 || fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, p.C, p.M, 0, false, 5, 0),
+                        "fed_round_small: too many clients for the centered-clipping scratch (use fed_round_small_fits to route)");
         }
     }
     if (fcfg.size() >= 22) {   // simulated Byzantine clients: fcfg[20] = attack kind (0 none, 1 sign_flip, 2 gaussian),
@@ -205,6 +208,21 @@ std::vector<int64_t> fed_round_small(
             p.attack_mask = am.data_ptr<uint8_t>();
         }
     }
+    if (p.agg_rule == 5) {   // centered clipping: fcfg[22] = radius tau, fcfg[23] = iterations L, state cc_center [M, P]
+        TORCH_CHECK(fcfg.size() >= 24, "fed_round_small: centered clipping needs fcfg {.., attack kind, attack scale, cclip_tau, cclip_iters}");
+        const double tau = fcfg[22], it = fcfg[23];
+        TORCH_CHECK(std::isfinite(tau) && tau > 0.0 && std::isfinite((float)tau) && (float)tau > 0.f,
+                    "fed_round_small: cclip_tau must be finite and > 0 in float32");
+        TORCH_CHECK(it >= 1.0 && it <= 100.0 && it == std::floor(it), "fed_round_small: cclip_iters must be an integer in [1, 100]");
+        TORCH_CHECK(cc_center.has_value() && cc_center->defined(), "fed_round_small: centered clipping needs the center tensor cc_center");
+        const Tensor& cc = *cc_center;
+        TORCH_CHECK(cc.is_cuda() && cc.device() == X.device() && cc.scalar_type() == torch::kFloat32 && cc.is_contiguous() && cc.dim() == 2 &&
+                        cc.size(0) == p.M && cc.size(1) == theta.size(1),
+                    "fed_round_small: cc_center must be a contiguous float32 [M, P] tensor on the device of X");
+        p.cc_tau = (double)(float)tau;   // fl32(τ) widened, as cclip_aggregate_slots
+        p.cc_iters = (int)it;
+        p.cc_center = cc.data_ptr<float>();
+    }
     fdb::SmallLaunchInfo info{};
     const int rc = fdb::fed_round_small_launch((int)kind, (int)din, (int)hid, (int)dout, p, cluster, cur_stream(), &info);
     TORCH_CHECK(rc != -1, "fed_round_small: MLP shape (", kind, ",", din, ",", hid, ",", dout, ") is not instantiated");
@@ -213,8 +231,8 @@ std::vector<int64_t> fed_round_small(
     return {info.cluster, info.threads, info.smem_bytes};
 }
 
-// agg_rule: 0 mean, 1 median, 2 trimmed mean, 3 geometric median, 4 Multi-Krum (the scratch each rule needs); attack_kind:
-// 0 none, 1 sign_flip, 2 gaussian (in the kernel), 3 alie, 4 ipm (never: the generic executor runs them)
+// agg_rule: 0 mean, 1 median, 2 trimmed mean, 3 geometric median, 4 Multi-Krum, 5 centered clipping (the scratch each rule
+// needs); attack_kind: 0 none, 1 sign_flip, 2 gaussian (in the kernel), 3 alie, 4 ipm (never: the generic executor runs them)
 bool fed_round_small_fits(int64_t kind, int64_t din, int64_t hid, int64_t dout, int64_t C, int64_t M, int64_t t_cur, bool server_opt,
                           int64_t agg_rule, int64_t attack_kind) {
     return fdb::fed_round_small_fits((int)kind, (int)din, (int)hid, (int)dout, (int)C, (int)M, (int)t_cur, server_opt, (int)agg_rule,
@@ -601,6 +619,75 @@ Tensor geomed_aggregate_slots(Tensor theta, Tensor cp, Tensor n, int64_t iters, 
                                                 0.999f, (float)eps, p0, p1, sp, mp, scratch.data_ptr(), cur_stream());
     TORCH_CHECK(rc != -2, "geomed_aggregate_slots: too many clients for the shared-memory staging of one column tile");
     TORCH_CHECK(rc == 0, "geomed_aggregate_slots: kernel launch failed");
+    if (sp) steps->add_((counts > 0).to(torch::kInt32));   // after the launch (same stream), as robust_aggregate_slots does
+    return counts;
+}
+
+// K23: centered clipping (ops/reference.py cclip_aggregate_slots_: iters clipping steps of radius tau around each slot's
+// center, its previous output) of the participants (n[c, m] > 0) of every slot of cp [C, M, P] into theta [M, >= P] (θ + v)
+// and center [M, P] (v); dmask [P] uint8 (or None) selects the entries of the distances.  The server optimizer arguments
+// are robust_aggregate_slots'.  Returns the participant counts [M] (float32).
+Tensor cclip_aggregate_slots(Tensor theta, Tensor cp, Tensor n, Tensor center, double tau, int64_t iters, int64_t opt_kind, double lr,
+                             double momentum, double eps, c10::optional<Tensor> s0, c10::optional<Tensor> s1,
+                             c10::optional<Tensor> steps, c10::optional<Tensor> mask, c10::optional<Tensor> dmask) {
+    CHECK_CUDA_F32(theta); CHECK_CUDA_F32(cp); CHECK_CUDA_F32(n); CHECK_CUDA_F32(center);
+    TORCH_CHECK(std::isfinite(tau) && tau > 0.0 && std::isfinite((float)tau) && (float)tau > 0.f,
+                "cclip_aggregate_slots: tau must be finite and > 0 in float32");
+    TORCH_CHECK(iters >= 1 && iters <= 100, "cclip_aggregate_slots: iters must be in [1, 100]");
+    TORCH_CHECK(cp.is_contiguous() && cp.dim() == 3, "cclip_aggregate_slots: cp must be a contiguous [C, M, P] tensor");
+    const int64_t C = cp.size(0), M = cp.size(1), P = cp.size(2);
+    TORCH_CHECK(C < (int64_t(1) << 31) && M <= 65535, "cclip_aggregate_slots: need C < 2^31 and M <= 65535");
+    TORCH_CHECK(n.device() == cp.device() && n.is_contiguous() && n.numel() == C * M,
+                "cclip_aggregate_slots: n must be a contiguous float32 [C, M] tensor on the device of cp");
+    TORCH_CHECK(theta.device() == cp.device() && theta.dim() == 2 && theta.size(0) == M && theta.size(1) >= P && theta.stride(1) == 1,
+                "cclip_aggregate_slots: theta must be [M, >= P] with unit column stride on the device of cp");
+    TORCH_CHECK(center.device() == cp.device() && center.is_contiguous() && center.dim() == 2 && center.size(0) == M &&
+                    center.size(1) == P,
+                "cclip_aggregate_slots: center must be a contiguous float32 [M, P] tensor on the device of cp");
+    const unsigned char* dp = nullptr;
+    if (dmask.has_value() && dmask->defined()) {
+        TORCH_CHECK(dmask->is_cuda() && dmask->device() == cp.device() && dmask->scalar_type() == torch::kUInt8 && dmask->is_contiguous() &&
+                    dmask->numel() == P, "cclip_aggregate_slots: dmask must be a contiguous uint8 [P] tensor on the device of cp");
+        dp = dmask->data_ptr<unsigned char>();
+    }
+    float *p0 = nullptr, *p1 = nullptr;
+    int* sp = nullptr;
+    const unsigned char* mp = nullptr;
+    if (opt_kind != 0) {
+        TORCH_CHECK(opt_kind >= 1 && opt_kind <= 4, "cclip_aggregate_slots: server optimizer kind must be 0..4");
+        for (const auto* t : {&s0, &s1}) {
+            if (t->has_value() && (*t)->defined()) {
+                CHECK_CUDA_F32(**t);
+                TORCH_CHECK((*t)->is_contiguous() && (*t)->dim() == 2 && (*t)->size(0) == M && (*t)->size(1) == P &&
+                            (*t)->device() == cp.device(),
+                            "cclip_aggregate_slots: optimizer state must be contiguous [M, P] on the device of cp");
+            }
+        }
+        p0 = opt_ptr<float>(s0); p1 = opt_ptr<float>(s1);
+        TORCH_CHECK(p0 || (opt_kind == 1 && momentum == 0.0), "cclip_aggregate_slots: this optimizer needs s0");
+        TORCH_CHECK(p1 || opt_kind == 1 || opt_kind == 3, "cclip_aggregate_slots: this optimizer needs s1");
+        TORCH_CHECK(steps.has_value() && steps->defined(), "cclip_aggregate_slots: a server optimizer needs the step counters");
+        CHECK_CUDA_I32(*steps);
+        TORCH_CHECK(steps->is_contiguous() && steps->numel() == M && steps->device() == cp.device(),
+                    "cclip_aggregate_slots: steps must be a contiguous int32 [M] tensor on the device of cp");
+        sp = steps->data_ptr<int>();
+        if (mask.has_value() && mask->defined()) {
+            TORCH_CHECK(mask->is_cuda() && mask->device() == cp.device() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                        mask->numel() == P, "cclip_aggregate_slots: mask must be a contiguous uint8 [P] tensor on the device of cp");
+            mp = mask->data_ptr<unsigned char>();
+        }
+    }
+    c10::cuda::CUDAGuard guard(cp.device());
+    auto counts = (n.view({C, M}) > 0).sum(0).to(torch::kFloat32);
+    const int64_t words = (fdb::cclip_scratch_bytes((int)C, (int)M, P) + 7) / 8;
+    auto scratch = torch::empty({std::max<int64_t>(words, 1)}, cp.options().dtype(torch::kFloat64));
+    const double tau_f = (double)(float)tau;   // fl32(τ) widened, as the fused kernel's fcfg
+    const int rc = fdb::cclip_aggregate_launch(theta.data_ptr<float>(), theta.stride(0), cp.data_ptr<float>(), n.data_ptr<float>(),
+                                               center.data_ptr<float>(), (int)C, (int)M, P, (int)iters, tau_f, dp, (int)opt_kind,
+                                               (float)lr, (float)momentum, 0.9f, 0.999f, (float)eps, p0, p1, sp, mp, scratch.data_ptr(),
+                                               cur_stream());
+    TORCH_CHECK(rc != -2, "cclip_aggregate_slots: too many clients for the shared-memory staging of one column tile");
+    TORCH_CHECK(rc == 0, "cclip_aggregate_slots: kernel launch failed");
     if (sp) steps->add_((counts > 0).to(torch::kInt32));   // after the launch (same stream), as robust_aggregate_slots does
     return counts;
 }
@@ -1319,6 +1406,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("robust_aggregate_slots", &robust_aggregate_slots);
     m.def("geomed_aggregate_slots", &geomed_aggregate_slots);
     m.def("krum_aggregate_slots", &krum_aggregate_slots);
+    m.def("cclip_aggregate_slots", &cclip_aggregate_slots);
     m.def("eval_logits", &eval_logits);
     m.def("aue_sqerr", &aue_sqerr);
     m.def("ensemble_vote", &ensemble_vote);

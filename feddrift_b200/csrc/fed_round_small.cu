@@ -319,6 +319,86 @@ __device__ __noinline__ void krum_slots(const float* slot_s, const int* pairs_s,
     }
 }
 
+// Centered-clipping phase (RoundParams::agg_rule == 5), after the cluster barrier that makes every CTA's published uploads
+// visible (no median columns): CTA crank takes each slot m ≡ crank (mod G) (ops/reference.py cclip_aggregate_slots_) and
+// leaves θ_s[m] + v in its own part[m·P …] (only the slot's owner reads those entries of it).  The slot's n uploads are
+// copied over DSMEM in pair order into scratch [n][P] as d = fl32(x − θ_s[m]), followed by the clip factors [n], the pair
+// list [n], n and the NaN flag — the CTA's gbuf, C·(P + 2) + 4 floats (fed_round_small_fits checks it).  v starts from the
+// slot's center h_m in global memory, which only this CTA reads and writes (the owner of slot m never changes), and is
+// kept in part until the end.  Warps over rows for the fp64 distances, threads over columns for the update, every
+// operation rounded on its own as in the oracle; h_m ← v at the end.
+template <int P>
+__device__ __noinline__ void cclip_slots(const float* slot_s, const int* pairs_s, int npairs, const float* tot_s, const float* theta_s,
+                                         float* part, float* scratch, float* center, int C, int M, int G, int crank, int warp,
+                                         int NW, int lane, int iters, double tau) {
+    cg::cluster_group cluster = cg::this_cluster();
+    const int tid = threadIdx.x, nthreads = NW * 32;
+    float* D = scratch;
+    float* sf = D + (size_t)C * P;
+    int* lst = reinterpret_cast<int*>(sf + C);
+    int* n_s = lst + C;
+    int* nan_s = n_s + 1;
+    for (int m = crank; m < M; m += G) {
+        if (!(tot_s[m] > 0.f)) continue;
+        float* v = part + m * P;
+        const float* th = theta_s + m * P;
+        float* h = center + (size_t)m * P;
+        if (warp == 0) {   // the slot's pairs in pair order
+            int base = 0;
+            for (int i0 = 0; i0 < npairs; i0 += 32) {
+                const int i = i0 + lane;
+                const bool on = i < npairs && pairs_s[i] % M == m;
+                const unsigned bal = __ballot_sync(0xffffffffu, on);
+                if (on) lst[base + __popc(bal & ((1u << lane) - 1u))] = i;
+                base += __popc(bal);
+            }
+            if (lane == 0) { *n_s = base; *nan_s = 0; }
+        }
+        for (int pp = tid; pp < P; pp += nthreads) v[pp] = h[pp];
+        __syncthreads();
+        const int n = *n_s;
+        for (int idx = tid; idx < n * P; idx += nthreads) {
+            const int i = idx / P, pp = idx - i * P, pi = lst[i];
+            D[idx] = __fsub_rn(*(cluster.map_shared_rank(slot_s + (pi / G) * P + pp, pi % G)), th[pp]);
+        }
+        __syncthreads();
+        const float nf = (float)n;
+        for (int it = 0; it < iters; ++it) {
+            for (int i = warp; i < n; i += NW) {
+                double s = 0.0;
+                for (int pp = lane; pp < P; pp += 32) {
+                    const double d = (double)__fsub_rn(D[i * P + pp], v[pp]);
+                    s = fma(d, d, s);
+                }
+                s = warp_sum(s);
+                if (lane == 0) {
+                    if (isnan(s)) *nan_s = 1;
+                    sf[i] = isnan(s) ? 0.f : (float)fmin(1.0, tau / sqrt(s));
+                }
+            }
+            __syncthreads();
+            if (*nan_s) break;
+            for (int pp = tid; pp < P; pp += nthreads) {
+                const float vp = v[pp];
+                float acc = 0.f;
+                for (int i = 0; i < n; ++i) {
+                    const float si = sf[i];
+                    if (si != 0.f) acc = __fadd_rn(acc, __fmul_rn(si, __fsub_rn(D[i * P + pp], vp)));
+                }
+                v[pp] = __fadd_rn(vp, __fdiv_rn(acc, nf));
+            }
+            __syncthreads();
+        }
+        const bool nan = *nan_s != 0;
+        for (int pp = tid; pp < P; pp += nthreads) {
+            const float vp = nan ? __int_as_float(0x7FC00000) : v[pp];
+            h[pp] = vp;
+            v[pp] = nan ? vp : __fadd_rn(th[pp], vp);
+        }
+        __syncthreads();   // the next slot rewrites the scratch and the flags
+    }
+}
+
 // sample coordinates of element i of the current mini-batch
 struct BatchSel {
     int mode;        // 0/1: contiguous [lo, lo+n) of (tb, c);  2: list
@@ -343,7 +423,7 @@ __device__ __noinline__ void attack_upload(float* thl, const float* th0, int kin
 // kDefend: the robust-aggregation variant (p.def_bound > 0), a separate instantiation so that the undefended kernel keeps
 // its code and register allocation; kProx: the FedProx variant (p.prox_mu > 0) and kComp: the upload compression
 // (kCompQsgd when p.q_level > 0, kCompEfTopk when p.topk_k > 0) and kRobust: a median / trimmed-mean aggregation rule
-// or geometric median or Multi-Krum (p.agg_rule != 0), and kAttack: simulated Byzantine clients (p.attack_kind != 0),
+// or geometric median or Multi-Krum or centered clipping (p.agg_rule != 0), and kAttack: simulated Byzantine clients (p.attack_kind != 0),
 // separate for the same reason
 template <class Net, bool kDefend, bool kProx, int kComp, bool kRobust, bool kAttack>
 __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_kernel(const __grid_constant__ RoundParams p) {
@@ -814,6 +894,9 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                 if (p.agg_rule == 4) {   // Multi-Krum needs no median: CTA k selects and averages the slots m ≡ k (mod G)
                     krum_slots<P>(slot_s, pairs_s, npairs, tot_s, part_s + buf * MP, smem + L.gbuf, C, M, G, crank, warp, NW, lane,
                                   p.krum_f, p.krum_m);
+                } else if (p.agg_rule == 5) {   // centered clipping needs no median: CTA k clips the slots m ≡ k (mod G)
+                    cclip_slots<P>(slot_s, pairs_s, npairs, tot_s, theta_s, part_s + buf * MP, smem + L.gbuf, p.cc_center, C, M, G,
+                                   crank, warp, NW, lane, p.cc_iters, p.cc_tau);
                 } else {
                     robust_columns<P>(slot_s, pairs_s, npairs, tot_s, theta_s, part_s + buf * MP, smem + L.gbuf + warp * (P * 33),
                                       M, G, crank, warp, NW, lane, p.agg_rule != 2, p.trim_ratio);
@@ -830,7 +913,7 @@ __global__ void __launch_bounds__(SmallCfg<Net>::kThreads, 1) fed_round_small_ke
                     const int m = e / P;
                     if (tot_s[m] > 0.f) {
                         float v = 0.f;
-                        if constexpr (kRobust)   // the column's owner (geometric median, Multi-Krum: the slot's owner)
+                        if constexpr (kRobust)   // the column's owner (rules 3, 4 and 5: the slot's owner)
                             v = *(cluster.map_shared_rank(part_s + buf * MP + e, p.agg_rule >= 3 ? m % G : e % G));
                         else for (int rk = 0; rk < G; ++rk) v += *(cluster.map_shared_rank(part_s + buf * MP + e, rk));
                         if (p.sopt_kind) {
@@ -1158,17 +1241,18 @@ static int fits_round(int C, int M, bool server_opt) {
 }
 
 // 1 when the fused kernel can run this federation: instantiated shape, t_cur < kTmax, shared-memory layout (with the server
-// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule (agg_rule 1..4) 2·C ≤ 33·P (a slot's
+// optimizer state when server_opt) within 227 KB, and under a robust aggregation rule (agg_rule 1..5) 2·C ≤ 33·P (a slot's
 // uploads and their ranked copy fit the ranking warp's gbuf); the geometric median (3) also needs C·(P + 2) + 4 ≤ the
 // CTA's gbuf (a slot's uploads, weights and pair list), Multi-Krum (4) C·(P + 4·warps + 4) + 4 ≤ it (a slot's uploads,
-// per-warp fp64 distance and sorted rows, fp64 scores, pair list and selection flags).  attack_kind 3 (alie) and 4 (ipm)
-// need statistics over other CTAs' pairs before the defense runs, so they go to the generic executor (K22)
+// per-warp fp64 distance and sorted rows, fp64 scores, pair list and selection flags), centered clipping (5) the geometric
+// median's C·(P + 2) + 4 (a slot's update rows, clip factors and pair list).  attack_kind 3 (alie) and 4 (ipm) need
+// statistics over other CTAs' pairs before the defense runs, so they go to the generic executor (K22)
 int fed_round_small_fits(int kind, int din, int hid, int dout, int C, int M, int t_cur, bool server_opt, int agg_rule, int attack_kind) {
     if (t_cur >= kTmax || attack_kind == kAttackAlie || attack_kind == kAttackIpm) return 0;
 #define FDB_CASE(K, I, H, O)                                                                                            \
     if (kind == K && din == I && (K == 0 || hid == H) && dout == O)                                                     \
         return fits_round<Mlp<K, I, H, O>>(C, M, server_opt) && (agg_rule == 0 || 2 * C <= 33 * Mlp<K, I, H, O>::P) && \
-               (agg_rule != 3 || (long long)C * (Mlp<K, I, H, O>::P + 2) + 4 <=                                          \
+               ((agg_rule != 3 && agg_rule != 5) || (long long)C * (Mlp<K, I, H, O>::P + 2) + 4 <=                      \
                                      (long long)SmallCfg<Mlp<K, I, H, O>>::kWarps * 33 * Mlp<K, I, H, O>::P) &&          \
                (agg_rule != 4 || (long long)C * (Mlp<K, I, H, O>::P + 4 * SmallCfg<Mlp<K, I, H, O>>::kWarps + 4) + 4 <= \
                                      (long long)SmallCfg<Mlp<K, I, H, O>>::kWarps * 33 * Mlp<K, I, H, O>::P);

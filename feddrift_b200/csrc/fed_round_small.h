@@ -60,6 +60,11 @@ struct RoundParams {
     // agg_rule 4: Multi-Krum (ops/reference.py krum_aggregate_slots_): the average of the min(krum_m, n) uploads whose
     // summed squared distances to their clamp(n − krum_f − 2, 1, n − 1) nearest neighbours are smallest
     int krum_f, krum_m;
+    // agg_rule 5: centered clipping (ops/reference.py cclip_aggregate_slots_): cc_iters clipping steps of radius cc_tau
+    // (fl32(τ) widened) around the slot's center cc_center [M, P], its previous output, which the slot's owner CTA rewrites
+    int cc_iters;
+    double cc_tau;
+    float* cc_center;
     // simulated Byzantine clients (attack_kind 0 = off, 1 sign_flip, 2 gaussian; ops/reference.py attack_slots_): after
     // compression, every pair of a client with attack_mask[c] != 0 uploads θ_m − s·(x − θ_m) or θ_m + s·gauss_hash(
     // attack_seed(seed, round), c·M + m, e) instead of x, s = attack_scale, before client_out, the defense and the rule

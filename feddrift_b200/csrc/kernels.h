@@ -51,6 +51,15 @@ int krum_aggregate_launch(float* theta, long long t_stride, const float* cp, con
                           int mkeep, const unsigned char* dmask, int opt_kind, float lr, float momentum, float b1, float b2,
                           float eps, float* s0, float* s1, const int* steps, const unsigned char* mask, void* scratch,
                           cudaStream_t stream);
+// robust_agg.cu (K23): centered clipping (iters clipping steps around center [M, P], the slots' previous outputs, radius
+// tau = fl32(τ) widened; dmask [P] uint8 or null: the entries in the distances) of the same participants into theta (θ + v)
+// and center (v), server step as K19.  scratch holds cclip_scratch_bytes(C, M, P) bytes (8-byte aligned).  -2: C too large
+// for the staging tile
+long long cclip_scratch_bytes(int C, int M, long long P);
+int cclip_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, float* center, int C, int M,
+                           long long P, int iters, double tau, const unsigned char* dmask, int opt_kind, float lr, float momentum,
+                           float b1, float b2, float eps, float* s0, float* s1, const int* steps, const unsigned char* mask,
+                           void* scratch, cudaStream_t stream);
 // attack.cu (K22): simulated Byzantine clients of rows [C, M, P] against theta + m·t_stride: every attacker pair
 // (attackers[c] != 0, n[c·M + m] > 0) uploads the kind's poisoned value (1 sign_flip, 2 gaussian with gauss_hash(seed,
 // c·M + m, e), 3 alie, 4 ipm; scale s > 0) on the entries with mask != 0 (mask may be nullptr).  -5: bad kind or scale

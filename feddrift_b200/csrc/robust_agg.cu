@@ -38,6 +38,17 @@
 //                  phase (server step included).
 // The participants' rows are read once (the store pass reads the m_eff selected ones again).  No float atomics and a grid
 // fixed by the device and the shape, so every launch gives the same bits.
+//
+// K23: centered clipping (ops/reference.py cclip_aggregate_slots_ is the definition) of the same participants around the
+// slot's state h_m (center [M, P]), as L + 1 passes that share K19's compaction, tile staging and store phase:
+//   pass 1 … L    per tile, v^(l−1) (pass 1: h read back; later v^(l−2) + fl32(Σ_i fl32(s_i·u_i) / n) from the clip factors
+//                 of the previous finish step, written over h in place so that the next pass reads it), then each row's
+//                 fp64 partial Σ fl32(fl32(x − θ) − v)² over the tile's trainable columns, warp per row, accumulated per
+//                 CTA in tile order and stored to [M, gridX, C]; cclip_finish_kernel sums them in CTA order into r_i²,
+//                 s_i = fl32(min(1, τ / r_i)) (float64) and marks the slot NaN on a NaN distance;
+//   pass L + 1    v^L, θ_m + v^L into θ_m through the store phase (server step included) and v^L into h_m.
+// The participants' rows are read L + 1 times.  No float atomics and a grid that depends only on the device and the shape,
+// so every launch gives the same bits.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -506,6 +517,135 @@ __global__ void __launch_bounds__(kThreads) krum_store_kernel(float* __restrict_
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------- K23
+struct CclipState {
+    float* h;       // [M, P] the slots' centers; holds the iterate v between passes
+    double* part;   // [M, gridX, C] per-CTA partial squared distances of the participants (compacted order)
+    float* s;       // [M, C] clip factors of the last finish step
+    int* nan;       // [M] 1: a NaN distance, the slot becomes NaN
+};
+
+// bytes of dynamic shared memory of cclip_pass_kernel: distance accumulators [C] (double), tile [C][T + 1], participant
+// list [C], clip factors [C], the tile's θ and v [2T]
+inline size_t cclip_smem_bytes(int C, int T) {
+    return (size_t)C * sizeof(double) + ((size_t)C * (T + 1) + 2 * (size_t)C + 2 * (size_t)T) * sizeof(float) + 16;
+}
+
+// One pass of K23 over the column tiles of each slot (grid (gridX, M), persistent like K19).  The first pass starts from
+// v⁰ = h; later passes form v from the clip factors of the previous finish step; the last pass stores θ + v into θ_m and
+// v into h_m.
+__global__ void __launch_bounds__(kThreads) cclip_pass_kernel(float* __restrict__ theta, long long t_stride,
+                                                             const float* __restrict__ cp, const float* __restrict__ n, int C,
+                                                             int M, long long P, int T, bool first, bool last,
+                                                             const unsigned char* __restrict__ dmask, RobustOpt so,
+                                                             CclipState cs) {
+    extern __shared__ __align__(16) float sm[];
+    double* dacc = reinterpret_cast<double*>(sm);             // [C] this CTA's partial distances
+    float* tile = reinterpret_cast<float*>(dacc + C);         // [nrows][T + 1]
+    int* rows = reinterpret_cast<int*>(tile + (size_t)C * (T + 1));
+    float* sf = reinterpret_cast<float*>(rows + C);            // [C] clip factors
+    float* thv = sf + C;                                       // [T] the tile's θ
+    float* res = thv + T;                                      // [T] the tile's v
+    __shared__ int cnt_s;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int m = blockIdx.y;
+    const int cnt = compact_participants(n, C, M, m, rows, &cnt_s);
+    if (cnt == 0) return;
+    const bool nan = !first && cs.nan[m] != 0;
+    if (nan && !last) return;   // nothing left to iterate: the last pass writes NaN
+    float bc1, bc2;
+    server_bias_corrections(so, m, &bc1, &bc2);
+    float* out = theta + (size_t)m * t_stride;
+    float* hm = cs.h + (size_t)m * P;
+    const long long ntiles = (P + T - 1) / T;
+    if (nan) {   // last pass of a NaN slot: no rows to read
+        const float q = __int_as_float(0x7FC00000);
+        for (long long tile_i = blockIdx.x; tile_i < ntiles; tile_i += gridDim.x)
+            for (int j = tid; j < T && tile_i * T + j < P; j += kThreads) {
+                const long long e = tile_i * T + j;
+                store_entry(out, e, q, so, (size_t)m, P, bc1, bc2);
+                hm[e] = q;
+            }
+        return;
+    }
+    for (int i = tid; i < cnt; i += kThreads) {
+        dacc[i] = 0.0;
+        if (!first) sf[i] = cs.s[(size_t)m * C + i];
+    }
+    const float nf = (float)cnt;
+    const size_t rstride = (size_t)M * P;
+    const int pitch = T + 1;
+    const bool vec = ((P & 3) == 0) && ((((uintptr_t)cp) & 15) == 0);
+    __syncthreads();
+
+    for (long long tile_i = blockIdx.x; tile_i < ntiles; tile_i += gridDim.x) {
+        const long long col0 = tile_i * T;
+        const int tw = (int)min((long long)T, P - col0);
+        stage_tile(tile, cp, rows, cnt, rstride, m, P, col0, T, tw, vec);
+        __syncthreads();
+        // ---- v of the tile: h, or v + fl32(fl32(Σ_i fl32(s_i·u_i)) / n) in client order over the rows with s_i != 0
+        for (int j = tid; j < tw; j += kThreads) {
+            const long long e = col0 + j;
+            const float th = out[e];
+            float v = hm[e];
+            if (!first) {
+                float acc = 0.f;
+                for (int i = 0; i < cnt; ++i) {
+                    const float si = sf[i];
+                    if (si != 0.f) acc = __fadd_rn(acc, __fmul_rn(si, __fsub_rn(__fsub_rn(tile[(size_t)i * pitch + j], th), v)));
+                }
+                v = __fadd_rn(v, __fdiv_rn(acc, nf));
+            }
+            thv[j] = th;
+            res[j] = v;
+            if (last) {
+                store_entry(out, e, __fadd_rn(th, v), so, (size_t)m, P, bc1, bc2);
+                hm[e] = v;
+            } else if (!first) {
+                hm[e] = v;   // the next pass starts from this iterate
+            }
+        }
+        if (!last) {
+            __syncthreads();
+            // ---- squared distances of u = fl32(fl32(x − θ) − v) over the tile's trainable columns, warp per row
+            for (int i = warp; i < cnt; i += kWarps) {
+                double s = 0.0;
+                for (int j = lane; j < tw; j += 32)
+                    if (!dmask || dmask[col0 + j]) {
+                        const double d = (double)__fsub_rn(__fsub_rn(tile[(size_t)i * pitch + j], thv[j]), res[j]);
+                        s = fma(d, d, s);
+                    }
+                s = warp_sum(s);
+                if (lane == 0) dacc[i] += s;
+            }
+        }
+        __syncthreads();   // the next tile overwrites tile / thv / res
+    }
+    if (!last)
+        for (int i = tid; i < cnt; i += kThreads) cs.part[((size_t)m * gridDim.x + blockIdx.x) * C + i] = dacc[i];
+}
+
+// After a distance pass: r_i² = the CTA partials summed in CTA order, s_i = fl32(min(1, τ / r_i)) (float64; r = 0 gives 1,
+// r = +∞ gives 0); a NaN distance marks the slot NaN.  One CTA per slot.
+__global__ void __launch_bounds__(kThreads) cclip_finish_kernel(const float* __restrict__ n, int C, int M, int gx, double tau,
+                                                               CclipState cs) {
+    extern __shared__ __align__(16) float sm[];
+    int* rows = reinterpret_cast<int*>(sm);
+    __shared__ int cnt_s, nan_s;
+    const int m = blockIdx.x;
+    if (threadIdx.x == 0) nan_s = 0;
+    const int cnt = compact_participants(n, C, M, m, rows, &cnt_s);
+    if (cnt == 0 || cs.nan[m] != 0) return;
+    for (int i = threadIdx.x; i < cnt; i += kThreads) {
+        double r2 = 0.0;
+        for (int b = 0; b < gx; ++b) r2 += cs.part[((size_t)m * gx + b) * C + i];
+        if (isnan(r2)) nan_s = 1;
+        cs.s[(size_t)m * C + i] = isnan(r2) ? 0.f : (float)fmin(1.0, tau / sqrt(r2));
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && nan_s) cs.nan[m] = 1;
+}
+
 }  // namespace
 
 int robust_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, int C, int M, long long P,
@@ -638,6 +778,59 @@ int krum_aggregate_launch(float* theta, long long t_stride, const float* cp, con
     const dim3 sgrid((unsigned)persistent_grid_x((P + kThreads - 1) / kThreads, M), (unsigned)M);
     krum_store_kernel<<<sgrid, kThreads, (size_t)C * sizeof(int), stream>>>(theta, t_stride, cp, C, M, P, sel, selcnt, so);
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
+}
+
+namespace {
+inline int cclip_tile(int C) {
+    return tile_width(C, [](int c, int t) { return (cclip_smem_bytes(c, t) + 3) / 4; });
+}
+}  // namespace
+
+long long cclip_scratch_bytes(int C, int M, long long P) {
+    if (C <= 0 || M <= 0 || P <= 0) return 0;
+    const int T = cclip_tile(C);
+    const long long gx = persistent_grid_x((P + T - 1) / T, M);
+    return (long long)M * gx * C * 8 + (long long)M * C * 4 + (long long)M * 4;
+}
+
+int cclip_aggregate_launch(float* theta, long long t_stride, const float* cp, const float* n, float* center, int C, int M,
+                           long long P, int iters, double tau, const unsigned char* dmask, int opt_kind, float lr, float momentum,
+                           float b1, float b2, float eps, float* s0, float* s1, const int* steps, const unsigned char* mask,
+                           void* scratch, cudaStream_t stream) {
+    if (C <= 0 || M <= 0 || P <= 0) return 0;
+    if (M > 65535) return -5;
+    const int T = cclip_tile(C);
+    const size_t smem = cclip_smem_bytes(C, T);
+    if (smem > 227 * 1024) return -2;
+    if (smem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute(cclip_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return -3;
+    }
+    const size_t fsmem = (size_t)C * sizeof(int);
+    if (fsmem > 227 * 1024) return -2;
+    if (fsmem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute(cclip_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);
+        if (e != cudaSuccess) return -3;
+    }
+    const int gx = persistent_grid_x((P + T - 1) / T, M);
+    char* sp = static_cast<char*>(scratch);
+    CclipState cs;
+    cs.h = center;
+    cs.part = reinterpret_cast<double*>(sp);              sp += (size_t)M * gx * C * 8;
+    cs.s = reinterpret_cast<float*>(sp);                  sp += (size_t)M * C * 4;
+    cs.nan = reinterpret_cast<int*>(sp);
+    if (cudaMemsetAsync(cs.nan, 0, (size_t)M * sizeof(int), stream) != cudaSuccess) return -4;
+    const RobustOpt none{0, 0.f, 0.f, b1, b2, eps, nullptr, nullptr, nullptr, nullptr};
+    const RobustOpt so{opt_kind, lr, momentum, b1, b2, eps, s0, s1, steps, mask};
+    const dim3 grid((unsigned)gx, (unsigned)M);
+    for (int t = 1; t <= iters + 1; ++t) {
+        const bool last = t == iters + 1;
+        cclip_pass_kernel<<<grid, kThreads, smem, stream>>>(theta, t_stride, cp, n, C, M, P, T, t == 1, last, dmask,
+                                                            last ? so : none, cs);
+        if (!last) cclip_finish_kernel<<<M, kThreads, fsmem, stream>>>(n, C, M, gx, tau, cs);
+        if (cudaGetLastError() != cudaSuccess) return -4;
+    }
+    return 0;
 }
 
 }  // namespace fdb

@@ -34,7 +34,7 @@ from ..data import changepoints as cpmod
 from ..data.drift import DEFAULT_DELTAS, DriftData
 from ..models import utils as mutils
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, attack_params, attack_seed, attacker_clients, compress_seed,
+from ..ops.reference import (aggregation_params, attack_params, attack_seed, attacker_clients, cclip_params, compress_seed,
                              compression_params, geomed_params, krum_params, prox_mu_param, topk_k, topk_ratio_param)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ModelBank
@@ -427,12 +427,19 @@ class _BaseAggregator:
         gm_iters, gm_nu = geomed_params(getattr(args, "geomed_iters", 4), getattr(args, "geomed_nu", 1e-6))
         # Multi-Krum (--krum_f / --krum_m, validated whatever the rule) carries (rule, β, f, m), distances as above
         krum_f, krum_m = krum_params(getattr(args, "krum_f", 1), getattr(args, "krum_m", 1))
+        # centered clipping (--cclip_tau / --cclip_iters, validated whatever the rule) carries (rule, β, τ, L), distances as
+        # above; the aggregator is rebuilt every time step, so the bank's per-slot centers start at zero here
+        cc_tau, cc_iters = cclip_params(getattr(args, "cclip_tau", 1.0), getattr(args, "cclip_iters", 1))
+        self.bank.cclip_center = None
         if rule == "mean":
             self.agg_rule = None
         elif rule == "geometric_median":
             self.agg_rule = (rule, beta, gm_iters, gm_nu)
         elif rule == "multi_krum":
             self.agg_rule = (rule, beta, krum_f, krum_m)
+        elif rule == "centered_clip":
+            self.agg_rule = (rule, beta, cc_tau, cc_iters)
+            self.bank.cclip_center = torch.zeros(self.bank.num_models, self.bank.P, dtype=torch.float32, device=self.device)
         else:
             self.agg_rule = (rule, beta)
         # upload compression (--compression qsgd): each arriving upload is quantized against bank.theta[m]; its draws follow
@@ -532,7 +539,10 @@ class _BaseAggregator:
             a = self.args
             seed = int(getattr(a, "dummy_arg", 0)) * 7919 + 13 + 1000003 * int(getattr(a, "curr_train_iteration", 0) or 0)
             self.defense.defend_slots_(self.upload, self.bank.theta, n, self.defense_mask, seed, self._defense_round)
-        if self.agg_rule is not None and self.agg_rule[0] in ("geometric_median", "multi_krum"):
+        if self.agg_rule is not None and self.agg_rule[0] == "centered_clip":
+            ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt, self.agg_rule, mask=self.defense_mask,
+                                   center=self.bank.cclip_center)
+        elif self.agg_rule is not None and self.agg_rule[0] in ("geometric_median", "multi_krum"):
             ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt, self.agg_rule, mask=self.defense_mask)
         else:
             ops.cluster_aggregate_(self.bank.theta, self.upload, n, self.bank.server_opt, self.agg_rule)

@@ -57,6 +57,14 @@ CONFIGS = {
                                                         concept_drift_algo_arg="H_A_C_1_10_0", concept_num=4, change_points="A",
                                                         sample_num=100, batch_size=500, comm_round=40,
                                                         aggregation_rule="multi_krum", krum_f=1, krum_m=1),
+    # config 2 with centered clipping (τ = 0.3, L = 1) as the cluster aggregation rule.  τ from a CPU run of config 2 (3 time
+    # steps × 10 rounds, 3,000 uploads): the honest update distances ‖x − θ‖ had median 0.16, 99th percentile 0.298 and
+    # maximum 0.301, so τ clips almost no honest update while bounding an attacker's pull to 0.3/n per round
+    "cfg2c_sea_fnn_100clients_cclip_feddrift": dict(model="fnn", dataset="sea", client_num_in_total=100, client_num_per_round=100,
+                                                    concept_drift_algo="softcluster", concept_drift_algo_arg="H_A_C_1_10_0",
+                                                    concept_num=4, change_points="A", sample_num=100, batch_size=500,
+                                                    comm_round=40, aggregation_rule="centered_clip", cclip_tau=0.3,
+                                                    cclip_iters=1),
     # config 2 with 20 colluding ALIE clients ("A Little Is Enough", z = 1) against the coordinate-wise median
     "cfg2a_sea_fnn_100clients_alie_median_feddrift": dict(model="fnn", dataset="sea", client_num_in_total=100,
                                                           client_num_per_round=100, concept_drift_algo="softcluster",

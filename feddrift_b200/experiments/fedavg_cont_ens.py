@@ -68,7 +68,8 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--topk_ratio", type=float, default=0.01, help="eftopk: fraction ρ of the trainable entries kept, 0 < ρ <= 1")
     # Byzantine-robust cluster aggregation (Yin et al., 2018): the coordinate-wise median or β-trimmed mean of the slot's
     # uploads (after compression and the defense), each participant counted once, instead of the weighted average
-    a("--aggregation_rule", type=str, default="mean", choices=["mean", "median", "trimmed_mean", "geometric_median", "multi_krum"])
+    a("--aggregation_rule", type=str, default="mean",
+      choices=["mean", "median", "trimmed_mean", "geometric_median", "multi_krum", "centered_clip"])
     a("--trim_ratio", type=float, default=0.1, help="trimmed_mean: fraction β dropped at each end, 0 <= β < 0.5")
     # geometric median (RFA, Pillutla et al.): smoothed Weiszfeld steps from the coordinate-wise median
     a("--geomed_iters", type=int, default=4, help="geometric_median: Weiszfeld iterations R, 1..100")
@@ -77,6 +78,10 @@ def add_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     # rule with one name, --krum_m 1 is plain Krum
     a("--krum_f", type=int, default=1, help="multi_krum: Byzantine uploads f assumed per slot, 0..65535")
     a("--krum_m", type=int, default=1, help="multi_krum: uploads m averaged, 1..65535 (1: Krum)")
+    # centered clipping (Karimireddy, He & Jaggi, 2021): every update is clipped to radius τ around the slot's previous
+    # aggregate and the clipped updates are averaged, L times; the center is reset at every time step
+    a("--cclip_tau", type=float, default=1.0, help="centered_clip: clipping radius τ > 0")
+    a("--cclip_iters", type=int, default=1, help="centered_clip: clipping iterations L, 1..100")
     # simulated Byzantine clients: a fixed set of --attack_clients clients poisons its uploads after compression (sign_flip:
     # the reversed update, gaussian: noise around the model, alie: "A Little Is Enough", ipm: inner-product manipulation)
     a("--attack_type", type=str, default="none", choices=["none", "sign_flip", "gaussian", "alie", "ipm"])

@@ -23,6 +23,7 @@ Kernel map (SURVEY §2.9 numbering):
   K20 geomed_aggregate_slots_ (geometric median)        csrc/robust_agg.cu
   K21 krum_aggregate_slots_ (Multi-Krum)                csrc/robust_agg.cu
   K22 attack_slots_ (simulated Byzantine clients)       csrc/attack.cu
+  K23 cclip_aggregate_slots_ (centered clipping)        csrc/robust_agg.cu
 """
 from __future__ import annotations
 
@@ -54,14 +55,20 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
 
 
 # ----------------------------------------------------------------------------- K1
-def cluster_aggregate_(theta, client_params, n, server_opt=None, rule=None, mask=None):
+def cluster_aggregate_(theta, client_params, n, server_opt=None, rule=None, mask=None, center=None):
     """K1: θ_m ← weighted mean of ``client_params[:, m]`` for every slot with total weight > 0; returns the totals [M].
     ``server_opt`` (``server_opt.SlotServerOpt``) then steps each such slot on θ_m − avg_m with its own state.
     ``rule`` = ``(aggregation_rule, trim_ratio)`` with rule 'median' or 'trimmed_mean' replaces the weighted mean by K19
     (``robust_aggregate_slots_``: the participants n > 0 count once each) and returns the participant counts [M]; None or
     'mean' is the weighted mean above.  ``rule`` = ``('geometric_median', trim_ratio, iters, nu)`` takes K20
     (``geomed_aggregate_slots_``) instead, with ``mask`` the trainable entries its distances cover (None: all), and
-    ``('multi_krum', trim_ratio, f, m)`` takes K21 (``krum_aggregate_slots_``) with the same ``mask``."""
+    ``('multi_krum', trim_ratio, f, m)`` takes K21 (``krum_aggregate_slots_``) with the same ``mask``.
+    ``('centered_clip', trim_ratio, tau, iters)`` takes K23 (``cclip_aggregate_slots_``) with the same ``mask`` around
+    ``center`` [M, P], the slots' state, which it updates; it is required for this rule and ignored otherwise."""
+    if rule is not None and rule[0] == "centered_clip":
+        if center is None:
+            raise ValueError("cluster_aggregate_: centered_clip needs the slots' centers (center=)")
+        return cclip_aggregate_slots_(theta, client_params, n, center, rule[2], rule[3], server_opt, mask)
     if rule is not None and rule[0] == "geometric_median":
         return geomed_aggregate_slots_(theta, client_params, n, rule[2], rule[3], server_opt, mask)
     if rule is not None and rule[0] == "multi_krum":
@@ -149,6 +156,32 @@ def krum_aggregate_slots_(theta, uploads, n, f: int = 1, m: int = 1, server_opt=
         return ref.krum_aggregate_slots_(theta, uploads, n, f, m, mask)
     avg = theta.clone()
     counts = ref.krum_aggregate_slots_(avg, uploads, n, f, m, mask)
+    so = server_opt
+    ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
+    return counts
+
+
+def cclip_aggregate_slots_(theta, uploads, n, center, tau: float = 1.0, iters: int = 1, server_opt=None, mask=None):
+    """K23: θ_m ← θ_m + v_m, centered clipping (``iters`` steps of radius ``tau`` around the slot's center, its previous
+    output) of the updates ``uploads[c, m]`` − θ_m with ``n[c, m] > 0`` (each counted once) for every slot with a
+    participant, and ``center[m]`` ← v_m; ``theta`` may be a padded bank; ``mask`` [P] (bool, None = all) selects the
+    entries of the distances (BatchNorm statistics are clipped along but left out).  ``server_opt`` then steps each such
+    slot on θ_m − (θ_m + v_m) and advances its counter.  See ``reference.cclip_aggregate_slots_``; returns the participant
+    counts [M]."""
+    tau, iters = ref.cclip_params(tau, iters)
+    if native(theta, uploads):
+        nn = n.float().contiguous()
+        dm = None if mask is None else mask.reshape(-1)[: uploads.shape[2]].to(uploads.device, torch.uint8).contiguous()
+        if server_opt is None:
+            return _ext.load().cclip_aggregate_slots(theta, uploads.contiguous(), nn, center, tau, iters, 0, 0.0, 0.0, 1e-8,
+                                                     None, None, None, None, dm)
+        so = server_opt
+        return _ext.load().cclip_aggregate_slots(theta, uploads.contiguous(), nn, center, tau, iters, so.kind, so.lr, so.momentum,
+                                                 so.eps, so.s0, so.s1, so.step, so._mask_u8, dm)
+    if server_opt is None:
+        return ref.cclip_aggregate_slots_(theta, uploads, n, center, tau, iters, mask)
+    avg = theta.clone()
+    counts = ref.cclip_aggregate_slots_(avg, uploads, n, center, tau, iters, mask)
     so = server_opt
     ref.server_opt_slots_(theta, avg, counts > 0, so.opt, so.s0, so.s1, so.step, so.lr, so.momentum, so.eps, so.mask)
     return counts

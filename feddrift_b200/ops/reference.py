@@ -228,6 +228,10 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     rule by ``geomed_params``: the same, with ``geomed_aggregate_slots_`` (every entry is trainable in these MLPs).
     ``aggregation_rule`` 'multi_krum' with ``krum_f`` f (1) and ``krum_m`` m (1), validated whatever the rule by
     ``krum_params``: the same, with ``krum_aggregate_slots_``.
+    ``aggregation_rule`` 'centered_clip' with ``cclip_tau`` τ (1.0) and ``cclip_iters`` L (1), validated whatever the
+    rule by ``cclip_params``, and state ``cclip_center [M, P]`` (created zero when missing, updated in place like the
+    optimizer moments): the same, with ``cclip_aggregate_slots_`` around the round-start θ; the server optimizer steps on
+    θ_m − (θ_m + v).
     ``attack_type`` 'sign_flip'|'gaussian'|'alie'|'ipm' (absent or 'none': off) with ``attack_clients`` a (0) and
     ``attack_scale`` s (1.0), validated whatever the type by ``attack_params``, and ``attackers`` (bool/uint8 [C], absent:
     ``attacker_clients(C, a, 0)``, which must hold a clients): after compression and before ``client_out``, the defense
@@ -269,6 +273,9 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
     agg_rule, trim_ratio = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
     gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
     krum_f, krum_m = krum_params(st.get("krum_f", 1), st.get("krum_m", 1))
+    cc_tau, cc_iters = cclip_params(st.get("cclip_tau", 1.0), st.get("cclip_iters", 1))
+    if agg_rule == "centered_clip" and st.get("cclip_center") is None:
+        st["cclip_center"] = torch.zeros(M, P, dtype=torch.float32)
     atk_type, atk_a, atk_scale = attack_params(st.get("attack_type") or "none", st.get("attack_clients", 0),
                                                st.get("attack_scale", 1.0), C)
     attackers = attack_table(st.get("attackers"), C, atk_a)
@@ -357,6 +364,8 @@ def fed_round_small(st: Dict, rounds: int = 1) -> Dict[str, torch.Tensor]:
                 geomed_aggregate_slots_(avg, up, trained, gm_iters, gm_nu)
             elif agg_rule == "multi_krum":
                 krum_aggregate_slots_(avg, up, trained, krum_f, krum_m)
+            elif agg_rule == "centered_clip":
+                cclip_aggregate_slots_(avg, up, trained, st["cclip_center"], cc_tau, cc_iters)
             else:
                 robust_aggregate_slots_(avg, up, trained, agg_rule, trim_ratio)
         for m in range(M):
@@ -718,13 +727,13 @@ def topk_upload_bits(P_train: int, P_other: int, k: int) -> int:
 
 
 # Multi-Krum has one name: ``multi_krum`` with ``krum_m`` = 1 is plain Krum, and a bare ``krum`` is an unknown rule.
-AGGREGATION_RULES = ("mean", "median", "trimmed_mean", "geometric_median", "multi_krum")
+AGGREGATION_RULES = ("mean", "median", "trimmed_mean", "geometric_median", "multi_krum", "centered_clip")
 
 
 def aggregation_params(rule, trim_ratio) -> Tuple[str, float]:
     """Validated ``(--aggregation_rule, --trim_ratio)``.  The rule is one of ``mean`` (weighted FedAvg), ``median``,
-    ``trimmed_mean``, ``geometric_median`` or ``multi_krum``; β is checked whatever the rule and must be a finite number
-    with 0 ≤ β < 0.5.  Raises ``ValueError``."""
+    ``trimmed_mean``, ``geometric_median``, ``multi_krum`` or ``centered_clip``; β is checked whatever the rule and must
+    be a finite number with 0 ≤ β < 0.5.  Raises ``ValueError``."""
     rule = "mean" if rule is None else rule
     if rule not in AGGREGATION_RULES:
         raise ValueError(f"aggregation_rule must be one of {', '.join(AGGREGATION_RULES)} (got {rule!r})")
@@ -964,6 +973,84 @@ def krum_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch.T
         if len(sel) > 1:
             v = v / torch.tensor(float(len(sel)), dtype=torch.float32, device=dev)
         theta[s, :P] = v.to(theta.device)
+    return counts.to(theta.device)
+
+
+CCLIP_MAX_ITERS = 100
+
+
+def cclip_params(tau, iters) -> Tuple[float, int]:
+    """Validated ``(--cclip_tau, --cclip_iters)``, checked whatever the rule: τ a finite number > 0 whose float32 rounding
+    is finite and > 0, L an int with 1 ≤ L ≤ 100 (a bool is not a number or an int here).  Raises ``ValueError``."""
+    try:
+        t = None if isinstance(tau, bool) else float(tau)
+    except (TypeError, ValueError):
+        t = None
+    if t is None or not _F32_ZERO_AT < t < _F32_INF_AT:
+        raise ValueError(f"cclip_tau must be a finite number > 0 (got {tau!r})")
+    if isinstance(iters, bool) or not isinstance(iters, (int, np.integer)) or not 1 <= int(iters) <= CCLIP_MAX_ITERS:
+        raise ValueError(f"cclip_iters must be an int in [1, {CCLIP_MAX_ITERS}] (got {iters!r})")
+    return t, int(iters)
+
+
+def cclip_aggregate_slots_(theta: torch.Tensor, uploads: torch.Tensor, n: torch.Tensor, center: torch.Tensor,
+                           tau: float = 1.0, iters: int = 1, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Centered clipping (K23; Karimireddy, He & Jaggi, ICML 2021), in place on ``theta`` and ``center``.  For every slot m
+    the participants x_1…x_n are the rows c with ``n[c, m] > 0`` in ascending c, each counted once (the weights are
+    ignored, as in ``robust_aggregate_slots_``); ``theta`` may be a padded bank, θ_m = ``theta[m, :P]`` the round-start
+    model, and ``center [M, P]`` holds each slot's previous centered-clipping output h_m (the state carried from round to
+    round).
+
+    * d_ie = fl32(x_ie − θ_me) for every entry; v⁰ = h_m.
+    * Iteration l = 1…L (L = ``iters``): u_ie = fl32(d_ie − v_e); r_i² = Σ_e mask_e · (double) u_ie², summed in float64
+      over the trainable entries (``mask``, None = all, so BatchNorm statistics stay out); s_i = fl32(min(1, τ_f / r_i))
+      computed in float64 and rounded once, τ_f = fl32(τ) widened to double (r = 0 gives 1, r = +∞ gives 0); rows with
+      s_i = 0 are skipped; acc_e = Σ_i fl32(s_i · u_ie) in client order from 0, and v_e ← fl32(v_e + fl32(acc_e / n)) for
+      every entry (BatchNorm statistics included).
+    * θ_me ← fl32(θ_me + v_e) for every entry, and h_m ← v.
+
+    A NaN distance makes the slot NaN (0x7FC00000) in θ_m and h_m.  The float64 distance sums depend on the reduction
+    order, so the GPU matches this to a tolerance; when no row is clipped (every s_i = 1) the result is bit-identical.
+    Slots with n = 0 keep θ_m and h_m.  Returns the per-slot participant counts ``[M]`` (float32)."""
+    tau, L = cclip_params(tau, iters)
+    tau_d = float(np.float32(tau))
+    C, M, P = uploads.shape
+    dev = uploads.device
+    part = n.detach().reshape(C, M).to(dev) > 0
+    counts = part.sum(0).to(torch.float32)
+    keep = None if mask is None else mask.reshape(-1)[:P].to(dev, torch.bool)
+    zero64 = torch.zeros((), dtype=torch.float64, device=dev)
+    for m in range(M):
+        idx = part[:, m].nonzero().flatten()
+        k = int(idx.numel())
+        if k == 0:
+            continue
+        th = theta[m, :P].to(dev, torch.float32)
+        d = uploads[idx, m].to(torch.float32) - th
+        v = center[m].to(dev, torch.float32).clone()
+        div = torch.tensor(float(k), dtype=torch.float32, device=dev)
+        nan = False
+        for _ in range(L):
+            u = d - v
+            sq = u.double().square()
+            if keep is not None:
+                sq = torch.where(keep, sq, zero64)
+            r2 = sq.sum(1)
+            if bool(torch.isnan(r2).any()):
+                nan = True
+                break
+            s = torch.clamp(tau_d / torch.sqrt(r2), max=1.0).to(torch.float32)
+            acc = torch.zeros(P, dtype=torch.float32, device=dev)
+            for i in range(k):
+                if float(s[i]) != 0.0:
+                    acc = acc + s[i] * u[i]
+            v = v + acc / div
+        if nan:
+            v = torch.full((P,), _QNAN32, dtype=torch.float32, device=dev)
+            theta[m, :P] = v.to(theta.device)
+        else:
+            theta[m, :P] = (th + v).to(theta.device)
+        center[m] = v.to(center.device)
     return counts.to(theta.device)
 
 

@@ -12,7 +12,7 @@ from .reference import ATTACK_ID, attack_params, attack_table
 
 KIND_ID = {"lr": 0, "fnn": 1}
 MODE_ID = {"pool": 0, "time": 1, "index": 2}
-AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2, "geometric_median": 3, "multi_krum": 4}
+AGG_RULE_ID = {"mean": 0, "median": 1, "trimmed_mean": 2, "geometric_median": 3, "multi_krum": 4, "centered_clip": 5}
 LAUNCH_COUNT = {"fed_round_small": 0}
 
 
@@ -26,10 +26,10 @@ def fits(kind: str, din: int, hid: int, dout: int, C: int, M: int, t_cur: int, s
     """True when the fused kernel can run this federation at time step ``t_cur`` (instantiated MLP shape, ``t_cur`` below
     the kernel's plan-table limit, shared-memory layout — plus the ``[2, M, P]`` server optimizer state when
     ``server_opt`` — within 227 KB, and with a ``robust`` aggregation rule 2·C ≤ 33·P for the ranking scratch; ``rule``
-    'geometric_median' (implies ``robust``) also needs a slot's C uploads and weights in the CTA's gradient buffers, and
-    'multi_krum' a slot's C uploads with per-warp distance rows in them); the ``attack`` types 'alie' and 'ipm' need
-    statistics over every upload of a slot before the defense, so they never fit ('sign_flip' and 'gaussian' run in the
-    publish step); otherwise route to the generic executor."""
+    'geometric_median' (implies ``robust``) also needs a slot's C uploads and weights in the CTA's gradient buffers,
+    'multi_krum' a slot's C uploads with per-warp distance rows in them, and 'centered_clip' the geometric median's room);
+    the ``attack`` types 'alie' and 'ipm' need statistics over every upload of a slot before the defense, so they never fit
+    ('sign_flip' and 'gaussian' run in the publish step); otherwise route to the generic executor."""
     ext = _ext.load()
     if ext is None:
         return True   # CPU reference has no such limits
@@ -167,10 +167,11 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
     elif compression != "none":
         from .reference import compression_params
         compression_params(compression, 16, 512)   # raises for an unknown compression
-    from .reference import aggregation_params, geomed_params, krum_params
+    from .reference import aggregation_params, cclip_params, geomed_params, krum_params
     rule, beta = aggregation_params(st.get("aggregation_rule") or "mean", st.get("trim_ratio", 0.1))
     gm_iters, gm_nu = geomed_params(st.get("geomed_iters", 4), st.get("geomed_nu", 1e-6))
     krum_f, krum_m = krum_params(st.get("krum_f", 1), st.get("krum_m", 1))
+    cc_tau, cc_iters = cclip_params(st.get("cclip_tau", 1.0), st.get("cclip_iters", 1))
     if rule != "mean":   # robust aggregation rule (reference.fed_round_small documents the keys)
         if mg:
             raise ValueError("a robust aggregation rule (--aggregation_rule) is single-GPU only")
@@ -180,6 +181,8 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
             fcfg += [float(gm_iters), gm_nu]
         elif rule == "multi_krum":   # the geometric-median slots 16..17 are unread
             fcfg += [4.0, 1e-6, float(krum_f), float(krum_m)]
+        elif rule == "centered_clip":   # the geometric-median and Multi-Krum slots 16..19 are unread
+            fcfg += [4.0, 1e-6, 1.0, 1.0]
     atk, atk_a, atk_s = attack_params(st.get("attack_type") or "none", st.get("attack_clients", 0), st.get("attack_scale", 1.0),
                                       C)
     attack_mask = None
@@ -192,6 +195,13 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         # server optimizer ... Multi-Krum slots, unread when off (the rule slots hold the mean and valid parameters)
         fcfg += [1.0, 0.0, 1e-8, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.1, 4.0, 1e-6, 1.0, 1.0][len(fcfg) - 5:]
         fcfg += [float(ATTACK_ID[atk]), atk_s]
+    cc_center = None
+    if rule == "centered_clip":   # the slots' centers, read and rewritten in place (reference.fed_round_small)
+        cc_center = st.get("cclip_center")
+        if cc_center is None:
+            cc_center = st["cclip_center"] = torch.zeros(M, theta.shape[1], dtype=torch.float32, device=dev)
+        fcfg += [0.0, 1.0][len(fcfg) - 20:]   # attack slots, unread without one
+        fcfg += [cc_tau, float(cc_iters)]
     peer_metrics = []
     if mg and mg.get("metrics_ptrs") is not None:
         # every rank's LL staging area (symmetric); the kernel compacts this launch's rows into the plain metrics_out
@@ -205,7 +215,7 @@ def run_native(st: Dict, rounds: int, metrics_out: Optional[torch.Tensor] = None
         list(mg["inbox_ptrs"]) if mg else [], mg.get("error_flag") if mg else None,
         st.get("counters"), peer_metrics, [int(v) for v in st["host_io"]] if st.get("host_io") else [],
         cache["participation"], st.get("server_s0") if sopt else None, st.get("server_s1") if sopt else None,
-        st.get("server_step") if sopt else None, ef_res, attack_mask)
+        st.get("server_step") if sopt else None, ef_res, attack_mask, cc_center)
     if mg:
         mg["flag_base"] = int(mg["flag_base"]) + rounds
     if st.get("counters") is not None:

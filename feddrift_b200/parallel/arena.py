@@ -70,6 +70,9 @@ class ModelBank:
         # the clients' error-feedback residual [C, M, P] of --compression eftopk or None: residual built up against a slot's
         # old model means nothing for its new one, so reinit / copy zero the destination slot's column for every client
         self.ef_res = None
+        # the slots' centered-clipping state [M, P] of --aggregation_rule centered_clip (their previous outputs) or None: a
+        # slot that is re-initialised or overwritten starts from a zero center, so reinit / copy zero its row
+        self.cclip_center = None
         self.float_mask = torch.zeros(self.P, dtype=torch.bool)
         for _, _, dt, off, n in self.spec:
             self.float_mask[off:off + n] = bool(dt.is_floating_point)
@@ -103,6 +106,8 @@ class ModelBank:
                 self.server_opt.reset(dst)
             if self.ef_res is not None:
                 self.ef_res[:, dst].zero_()
+            if self.cclip_center is not None:
+                self.cclip_center[dst].zero_()
 
     def reinit(self, m: int) -> None:
         self.theta[m].copy_(self.init_row)
@@ -110,6 +115,8 @@ class ModelBank:
             self.server_opt.reset(m)
         if self.ef_res is not None:
             self.ef_res[:, m].zero_()
+        if self.cclip_center is not None:
+            self.cclip_center[m].zero_()
 
     def reset_parameters_random(self, m: int, generator: Optional[torch.Generator] = None) -> None:
         """Fresh (NOT reseeded) init — the IFCA 'hard' path at t=0 calls ``reset_parameters`` directly

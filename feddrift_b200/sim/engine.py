@@ -36,8 +36,9 @@ from ..drift.evaluator import Evaluator
 from ..models import utils as mutils
 from ..models.utils import create_model
 from ..core.robustness import make_defense
-from ..ops.reference import (aggregation_params, attack_params, attacker_clients, compression_params, geomed_params,
-                             krum_params, prox_mu_param, qsgd_upload_bits, topk_k, topk_ratio_param, topk_upload_bits)
+from ..ops.reference import (aggregation_params, attack_params, attacker_clients, cclip_params, compression_params,
+                             geomed_params, krum_params, prox_mu_param, qsgd_upload_bits, topk_k, topk_ratio_param,
+                             topk_upload_bits)
 from ..ops.server_opt import make_server_opt
 from ..parallel.arena import ClientArena, ModelBank
 from ..utils.metrics import MetricsSink, get_sink
@@ -54,7 +55,7 @@ DEFAULTS = dict(
     server_optimizer="none", server_lr=1.0, server_momentum=0.0, server_eps=1e-8,
     defense_type="none", norm_bound=5.0, stddev=0.025, fedprox_mu=0.0,
     compression="none", quantize_level=16, quantize_bucket=512, topk_ratio=0.01,
-    aggregation_rule="mean", trim_ratio=0.1, geomed_iters=4, geomed_nu=1e-6, krum_f=1, krum_m=1,
+    aggregation_rule="mean", trim_ratio=0.1, geomed_iters=4, geomed_nu=1e-6, krum_f=1, krum_m=1, cclip_tau=1.0, cclip_iters=1,
     attack_type="none", attack_clients=0, attack_scale=1.0,
 )
 
@@ -121,12 +122,18 @@ class DriftSim:
         gm_iters, gm_nu = geomed_params(getattr(args, "geomed_iters", 4), getattr(args, "geomed_nu", 1e-6))
         # Multi-Krum (--krum_f f / --krum_m m, validated whatever the rule) carries (rule, β, f, m)
         krum_f, krum_m = krum_params(getattr(args, "krum_f", 1), getattr(args, "krum_m", 1))
+        # centered clipping (--cclip_tau τ / --cclip_iters L, validated whatever the rule) carries (rule, β, τ, L); its state
+        # is the bank's per-slot center (ModelBank.cclip_center), zeroed at every time step
+        cc_tau, cc_iters = cclip_params(getattr(args, "cclip_tau", 1.0), getattr(args, "cclip_iters", 1))
         if rule == "mean":
             self.agg_rule = None
         elif rule == "geometric_median":
             self.agg_rule = (rule, beta, gm_iters, gm_nu)
         elif rule == "multi_krum":
             self.agg_rule = (rule, beta, krum_f, krum_m)
+        elif rule == "centered_clip":
+            self.agg_rule = (rule, beta, cc_tau, cc_iters)
+            self.bank.cclip_center = torch.zeros(self.M, self.bank.P, dtype=torch.float32, device=self.device)
         else:
             self.agg_rule = (rule, beta)
         # simulated Byzantine clients (--attack_type / --attack_clients a / --attack_scale s, validated whatever the type):
@@ -201,6 +208,8 @@ class DriftSim:
         self.clients.reset_optimizer()
         if self.bank.server_opt is not None:
             self.bank.server_opt.reset()
+        if self.bank.cclip_center is not None:
+            self.bank.cclip_center.zero_()
         self.algo.begin_step(t)
         self._small = None
         self._plan = None
@@ -269,6 +278,9 @@ class DriftSim:
                     self._small.update(geomed_iters=self.agg_rule[2], geomed_nu=self.agg_rule[3])
                 elif self.agg_rule[0] == "multi_krum":
                     self._small.update(krum_f=self.agg_rule[2], krum_m=self.agg_rule[3])
+                elif self.agg_rule[0] == "centered_clip":   # the bank's centers: the kernel reads and rewrites them in place
+                    self._small.update(cclip_tau=self.agg_rule[2], cclip_iters=self.agg_rule[3],
+                                       cclip_center=self.bank.cclip_center)
             if self.attack is not None:
                 self._small.update(attack_type=self.attack[0], attack_clients=int(self.attackers.sum()),
                                    attack_scale=self.attack[1], attackers=self._attackers_dev)
@@ -418,7 +430,7 @@ class DriftSim:
         cl = self.clients
         so = self.bank.server_opt
         snap = [(x, x.clone()) for x in (self.bank.theta, cl.m, cl.v, cl.vmax, cl.step, cl.ef_res, st.get("W"),
-                                         *(so.tensors() if so else ()))
+                                         self.bank.cclip_center, *(so.tensors() if so else ()))
                 if isinstance(x, torch.Tensor)]
         cnt = st.get("counters")
         cnt0 = cnt[0:1].clone() if isinstance(cnt, torch.Tensor) else None

@@ -17,7 +17,8 @@ architecture and for algorithms that must look at raw client updates before aggr
   simulated Byzantine clients (``sim.attack``) then replace their uploads in place (``ops.attack_slots_``, K22, clients
   ``sim.attackers``, entries ``sim.defense_mask``), so the hooks, the defense and the rule see the poisoned ones;
   a robust aggregation rule (``sim.agg_rule``) makes the same call take the coordinate-wise median / trimmed mean (K19)
-  or the geometric median (K20) or Multi-Krum (K21), both with distances over the trainable entries ``sim.defense_mask``;
+  or the geometric median (K20) or Multi-Krum (K21) or centered clipping (K23, around the bank's per-slot
+  ``cclip_center``), all three with distances over the trainable entries ``sim.defense_mask``;
 * evaluation: clients are grouped by the model they are scored with → one batched forward per (model, split), per-client
   sums by masked reduction on device, ONE host copy per block of rounds.
 
@@ -150,7 +151,10 @@ def run_rounds_generic(sim, rounds: int) -> Dict[str, torch.Tensor]:
                 _peer_aggregate(sim, world, rank)
             else:
                 rule = getattr(sim, "agg_rule", None)
-                if rule is not None and rule[0] in ("geometric_median", "multi_krum"):
+                if rule is not None and rule[0] == "centered_clip":
+                    ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule, mask=sim.defense_mask,
+                                           center=bank.cclip_center)
+                elif rule is not None and rule[0] in ("geometric_median", "multi_krum"):
                     ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule, mask=sim.defense_mask)
                 else:
                     ops.cluster_aggregate_(bank.theta, cl.params, cl.n, bank.server_opt, rule)
